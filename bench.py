@@ -1,11 +1,11 @@
 #!/usr/bin/env python
-"""bench.py — throughput of the hot path on N B200s of one node (driver contract).
+"""bench.py — throughput of the hot path on N H100s of one node.
 
 Two workloads:
   --workload clip (default): BASELINE's metric — clips/sec of a full 512x512 clip: 50 UNet evaluations (img2img with
       denoising 1.0, classifier-free guidance, PNDM) + VAE decode + image -> mel -> inverse mel -> 32-iteration
       Griffin-Lim, random-init SD-1.5 weights (BASELINE config 4: no network for the checkpoint), `--clips` clips
-      per GPU per step.  roofline = the tcgen05 GEMM/conv kernel (tensor bound).  The Griffin-Lim sub-benchmark of
+      per GPU per step.  roofline = the wgmma GEMM/conv kernel (tensor bound).  The Griffin-Lim sub-benchmark of
       configs[1] is run too and reported under "griffinlim" (its own HBM roofline = "GL HBM GB/s" of the metric).
   --workload gl: only BASELINE configs[1] — inverse-mel + 32-iteration Griffin-Lim, 512x512 mel, batch 64 per GPU.
   --workload riffuse: BASELINE configs[2] — ONE request through RiffusionPipeline.riffuse() (PIL in -> PIL out, seed image
@@ -23,6 +23,10 @@ gl workload: one "step" = one pass of the hot path over one batch of 64 syntheti
   cpu_baseline / --impl reference: the reference's own CPU arithmetic (installed torchaudio
            transforms built with the reference's arguments, oracle/torchaudio_ref.py) on all host
            cores, on a bounded sample (one clip per step).
+
+--dump-outputs DIR: after the timed steps, what the timed path returned in its last step is written as DIR/<name>.npy
+(float32, at most 64 MB in all; an output over its share is reduced to a fixed, seeded strided sample).  Inputs are
+seeded, so two builds run with the same arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -71,7 +75,25 @@ def peaks() -> dict:
     if f.exists():
         d = json.loads(f.read_text())
         return {"hbm_gbs": float(d["hbm_gbs"]), "source": "measured"}
-    return {"hbm_gbs": 6650.0, "source": "fallback"}
+    return {"hbm_gbs": 3350.0, "source": "fallback: H100 SXM data sheet"}
+
+
+DUMP_BUDGET_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir: str, arrays: dict) -> None:
+    """Write each output as out_dir/<name>.npy in float32.  An output larger than its share of DUMP_BUDGET_BYTES is
+    replaced by a fixed sample: every stride-th element of the flattened array from an offset drawn from a seeded RNG."""
+    d = Path(out_dir)
+    d.mkdir(parents=True, exist_ok=True)
+    share = DUMP_BUDGET_BYTES // max(len(arrays), 1)
+    for name, t in arrays.items():
+        a = (t.detach().float().cpu().numpy() if torch.is_tensor(t) else np.asarray(t, dtype=np.float32)).reshape(-1)
+        if a.nbytes > share:
+            stride = -(-a.size // (share // a.itemsize))
+            offset = int(np.random.default_rng(0).integers(stride))
+            a = a[offset::stride]
+        np.save(d / f"{name}.npy", np.ascontiguousarray(a, dtype=np.float32))
 
 
 class ClockSampler:
@@ -169,6 +191,8 @@ def main() -> None:
     ap.add_argument("--denoising", type=float, default=0.75, help="riffuse workload: img2img strength (0.75 -> 38 of 50 evals)")
     ap.add_argument("--clips", type=int, default=32, help="clips per GPU per step (clip workload)")
     ap.add_argument("--evals", type=int, default=50, help="scheduler steps = UNet evaluations per clip (denoising 1.0)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step to DIR/<name>.npy (rank 0)")
     args = ap.parse_args()
     if args.workload == "roundtrip" and args.clips == 32:
         args.clips = 16                      # BASELINE configs[4]: batch 128 on 8 GPUs
@@ -206,9 +230,9 @@ def main() -> None:
         print(json.dumps(line))
         return
 
-    # ------------------------------------------------------------------ B200 arm
+    # ------------------------------------------------------------------ GPU arm
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py: no CUDA device; the B200 arm has no CPU fallback (use --impl reference)")
+        raise SystemExit("bench.py: no CUDA device; the GPU arm has no CPU fallback (use --impl reference)")
     torch.cuda.set_device(local_rank)
     dev = torch.device("cuda", local_rank)
     dist = None
@@ -271,6 +295,8 @@ def main() -> None:
         sampler.start()
     ms_total = timed(step_device, args.steps)
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {"waveform": wave})
 
     # per-kernel CUDA-event timing of the same step (rank 0 reports)
     ms_cls = (ctypes.c_float * 3)()
@@ -357,7 +383,7 @@ def tensor_peaks() -> dict:
         d = json.loads(f.read_text())
         return {"burst": float(d["bf16_tflops"]), "sustained": float(d.get("bf16_tflops_sustained", d["bf16_tflops"])),
                 "source": "measured"}
-    return {"burst": 1590.0, "sustained": 1400.0, "source": "fallback"}
+    return {"burst": 989.0, "sustained": 989.0, "source": "fallback: H100 SXM data sheet, dense FP16"}
 
 
 def time_reference_clip(host_cores: int, budget_s: float = 25.0) -> dict:
@@ -387,7 +413,7 @@ def time_reference_clip(host_cores: int, budget_s: float = 25.0) -> dict:
 
 
 def clip_config(n_steps: int, n_evals: int, clips_per_gpu: int, workload: str = "clip", denoising: float = 1.0) -> dict:
-    """`config` of the clip-type workloads: shared by the B200 arm and the reference arm (the driver compares them)"""
+    """`config` of the clip-type workloads: shared by the GPU arm and the reference arm (the driver compares them)"""
     if workload == "roundtrip":
         name = (f"configs[4] audio->image->audio round trip: STFT + mel + uint8 image of {L_WAVE}-sample waveforms, VAE encode, "
                 f"{n_steps}-step img2img (denoising 1.0 -> {n_evals} CFG UNet evaluations, guidance 7, PNDM), VAE decode, image->mel + "
@@ -508,7 +534,7 @@ def main_clip(args) -> None:
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
     cores = os.cpu_count() or 1
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py: no CUDA device; the B200 arm has no CPU fallback (use --impl reference)")
+        raise SystemExit("bench.py: no CUDA device; the GPU arm has no CPU fallback (use --impl reference)")
     torch.cuda.set_device(local_rank)
     dev = torch.device("cuda", local_rank)
     dist = None
@@ -620,12 +646,14 @@ def main_clip(args) -> None:
             dist.barrier()
         torch.cuda.synchronize(dev)
 
+    last = [None]
+
     def timed(fn, steps):
         barrier()
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record(stream)
         for _ in range(steps):
-            fn()
+            last[0] = fn()
         e1.record(stream)
         barrier()
         ms = torch.tensor([e0.elapsed_time(e1)], device=dev)
@@ -642,11 +670,13 @@ def main_clip(args) -> None:
         sampler.start()
     ms_total = timed(step_device, args.steps)
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:      # before later steps reuse the CUDA-graph output buffers
+        dump_outputs(args.dump_outputs, {k: last[0][k] for k in ("images", "waveform", "latents", "latents_unscaled")})
     step_e2e()
     e2e_steps = min(args.steps, 5)       # the e2e loop repeats the whole step with host I/O: bounded so a large --steps stays within minutes
     ms_e2e = timed(step_e2e, e2e_steps)
 
-    # live tensor-core measurement: one eager (non-graph) step with CUDA events around every tcgen05 launch
+    # live tensor-core measurement: one eager (non-graph) step with CUDA events around every GEMM / conv launch
     pipe.use_cuda_graph = False
     step_device()
     lib.rf_tc_profile_begin()
@@ -666,7 +696,7 @@ def main_clip(args) -> None:
     achieved = tc_fl.value / (tc_ms.value / 1e3) / 1e12
     alg_tflop_step = B * (n_evals * 2 * UNET_TFLOP_PER_SAMPLE + VAE_DEC_TFLOP + (VAE_ENC_TFLOP if roundtrip else 0.0))
     roofline = {
-        "bound": "tensor", "kernel": "k_tc_gemm (tcgen05 GEMM / implicit-GEMM conv)", "achieved": achieved,
+        "bound": "tensor", "kernel": "k_tc_gemm (wgmma GEMM / implicit-GEMM conv)", "achieved": achieved,
         "peak": pk["sustained"], "unit": "TFLOP/s", "frac": achieved / pk["sustained"], "traffic": gemm_traffic(),
         "traffic_detail": gemm_traffic(detail=True),
         "peak_source": pk["source"] + " (sustained cuBLAS bf16: kernel timed inside a long step)",
@@ -755,7 +785,7 @@ def main_riffuse(args) -> None:
     world = int(os.environ.get("WORLD_SIZE", "1"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py: no CUDA device; the B200 arm has no CPU fallback (use --impl reference)")
+        raise SystemExit("bench.py: no CUDA device; the GPU arm has no CPU fallback (use --impl reference)")
     torch.cuda.set_device(local_rank)
     dev = torch.device("cuda", local_rank)
     dist = None
@@ -817,12 +847,14 @@ def main_riffuse(args) -> None:
             dist.barrier()
         torch.cuda.synchronize(dev)
 
+    last = [None]
+
     def timed(fn, steps):
         barrier()
         e0_, e1_ = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0_.record(stream)
         for _ in range(steps):
-            fn()
+            last[0] = fn()
         e1_.record(stream)
         barrier()
         ms = torch.tensor([e0_.elapsed_time(e1_)], device=dev)
@@ -839,6 +871,8 @@ def main_riffuse(args) -> None:
         sampler.start()
     ms_total = timed(step_device, args.steps)
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {"images": last[0][0]})
     step_e2e()
     ms_e2e = timed(step_e2e, args.steps)
     pipe.use_cuda_graph = False
@@ -856,7 +890,7 @@ def main_riffuse(args) -> None:
     pk = tensor_peaks()
     achieved = tc_fl.value / (tc_ms.value / 1e3) / 1e12
     alg = n_evals * 2 * UNET_TFLOP_PER_SAMPLE + VAE_DEC_TFLOP
-    roofline = {"bound": "tensor", "kernel": "k_tc_gemm (tcgen05 GEMM / implicit-GEMM conv)", "achieved": achieved,
+    roofline = {"bound": "tensor", "kernel": "k_tc_gemm (wgmma GEMM / implicit-GEMM conv)", "achieved": achieved,
                 "peak": pk["sustained"], "unit": "TFLOP/s", "frac": achieved / pk["sustained"], "traffic": gemm_traffic(),
                 "peak_source": pk["source"] + " (sustained cuBLAS bf16)", "kernel_ms_per_step": tc_ms.value,
                 "kernel_launches_per_step": tc_n.value, "kernel_share_of_step": tc_ms.value / ms_step,
@@ -885,9 +919,8 @@ def main_riffuse(args) -> None:
 
 
 def gemm_traffic(detail: bool = False):
-    """ncu dram__bytes_read + dram__bytes_write of the tensor-core kernel, average per launch over the 236 launches of one
-    CFG evaluation at the benchmarked batch (profiles/traffic_latest.json, from profiles/r02_eval32_launches_dram.csv);
-    detail=True: the whole record (bytes per evaluation, algorithmic bytes)"""
+    """DRAM bytes per launch of the tensor-core kernel from a committed traffic record (profiles/traffic_latest.json) when
+    one exists, else None; detail=True: the whole record (bytes per evaluation, algorithmic bytes)"""
     f = ROOT / "profiles" / "traffic_latest.json"
     try:
         rec = json.loads(f.read_text()).get("k_tc_gemm")

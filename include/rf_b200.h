@@ -1,5 +1,5 @@
 /*
- * rf_b200.h — C-ABI of the B200-native Riffusion hot paths (librf_b200.so).
+ * rf_b200.h — C-ABI of the H100-native Riffusion hot paths (librf_b200.so).
  *
  * The reference (riffusion/riffusion-hobby, pure Python) has no FFI; its seams are
  * duck-typed Python callables.  Each entry point below replaces the arithmetic behind
@@ -14,7 +14,7 @@
  *   - `stream` is a cudaStream_t passed as void* (NULL = legacy default stream);
  *   - all functions return 0 on success, non-zero on error; rf_last_error() returns a
  *     thread-local message.  There is NO CPU fallback: device entry points fail with
- *     RF_ERR_CUDA when no sm_100 device is usable;
+ *     RF_ERR_CUDA when no sm_90 device is usable;
  *   - no global mutable state: a plan is immutable after its first upload, so
  *     concurrent calls on different streams with different workspaces are safe
  *     (the reference shares one converter across a ThreadPool, riffusion/cli.py:172-204).

@@ -1,7 +1,7 @@
 """fp16-STORAGE emulation of the path-(b) oracle — TEST INFRASTRUCTURE ONLY (see oracle/__init__.py).
 
 Same arithmetic as oracle/unet_oracle.py / oracle/vae_oracle.py (it walks the very same nn.Modules and parameters), all
-math in fp32, but every tensor that the B200 kernels STORE in HBM as fp16 is rounded to fp16 here at the same point:
+math in fp32, but every tensor that the H100 kernels STORE in HBM as fp16 is rounded to fp16 here at the same point:
 after GroupNorm(+SiLU), LayerNorm, every conv / linear epilogue (bias, time-embedding bias, activation, residual add
 are applied in fp32 BEFORE the single rounding, as the fused epilogues do), Q / K / V, the softmax probabilities
 (rounded to fp16 before the P.V product, row sum taken from the rounded values) and the attention output.
@@ -11,7 +11,7 @@ Purpose (VERDICT r1 "meet or bound the 1e-3 tolerance"): the reference runs its 
 file, both asserted in tests/test_parity_bench_gpu.py:
   * rel_l2(emulation, fp32 oracle)  = what fp16 STORAGE alone costs for this network (the floor any fp16
     implementation, the reference's included, sits on);
-  * rel_l2(B200 kernels, emulation) = what the kernels add on top of that (accumulation order, MUFU approximations).
+  * rel_l2(H100 kernels, emulation) = what the kernels add on top of that (accumulation order, MUFU approximations).
 """
 from __future__ import annotations
 
@@ -200,7 +200,7 @@ def vae_decode(m, z, scale: float = 1.0):
 def img2img_loop_emul(unet_module, scheduler: uo.PNDMSchedulerOracle, text, uncond, init_latents, noise, strength: float,
                       num_inference_steps: int, guidance_scale: float, mask=None):
     """oracle.unet_oracle.img2img_loop (riffusion_pipeline.py:311-425) with fp16 storage at the points where the
-    B200 path stores fp16: UNet (unet_forward above), guided eps as three fp16 ops (what torch does on fp16 tensors,
+    GPU path stores fp16: UNet (unet_forward above), guided eps as three fp16 ops (what torch does on fp16 tensors,
     :411-415), multistep combination in fp32 with ONE rounding of the previous sample (rf_cfg_pndm_step_f16), fp16
     eps history, add_noise / mask blend with one rounding (rf_axpby_f16).  `noise` is the already-slerped tensor."""
     s = scheduler

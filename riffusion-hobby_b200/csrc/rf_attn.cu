@@ -1,18 +1,13 @@
-// Fused multi-head attention for the UNet's transformer blocks: O = softmax(Q K^T * scale) V per (image, head),
-// scores never leave the SM.  tcgen05 MMAs with TMEM accumulators, TMA-fed K / V^T tiles.
+// Fused multi-head attention for the UNet's and the text encoder's transformer blocks: O = softmax(Q K^T * scale) V per
+// (image, head); scores never leave the SM.  wgmma with register accumulators, TMA-fed Q / K / V^T tiles.
 //
-// Two passes over the keys instead of an online-softmax rescale:
-//   pass 1: S = Q K^T per 128-key tile -> running row maximum           (QK^T MMAs only)
-//   pass 2: S = Q K^T again, P = exp2((S - max) * scale*log2e) in fp16 -> shared memory, O += P V (TMEM
-//           accumulates across all key tiles, no correction step), row sums accumulated on the side;
-//           epilogue O / rowsum.
-// QK^T is computed twice (+1 MMA in 3 for d=40) but exp is evaluated once and O is never rescaled.
-//
-// CTA = 128 queries of one (image, head); 320 threads:
-//   warp 0      TMA producer (K tiles in pass 1, K + V^T tiles in pass 2), 1 thread
-//   warp 1      MMA issuer, 1 thread; TMEM allocation (512 columns: S0 | S1 | O)
-//   warps 2-5   softmax group A: even key tiles, one query row per thread (row == TMEM lane)
-//   warps 6-9   softmax group B: odd key tiles (ping-pong on the two S buffers / two P buffers)
+// CTA = 128 queries of one (image, head); 288 threads:
+//   warps 0-3 / 4-7  two consumer warpgroups, 64 query rows each.  Per 64-key tile: S = Q K^T (wgmma, both operands in
+//                    shared memory), online softmax in registers (running row maximum, the accumulator and row sum rescaled
+//                    when it grows), P rounded to fp16 and fed straight from registers as the A operand of O += P V.
+//   warp 8           TMA producer (one thread): Q once, then K / V^T tiles through an NS-deep mbarrier ring.
+// The row sums are accumulated from the fp16-rounded P that the P V product actually uses.
+// Causal mask (CLIP text encoder): key j is visible to query i only if j <= i.
 //
 // Replaces the baddbmm -> softmax -> bmm sequence of diffusers' CrossAttention (reached from
 // riffusion/riffusion_pipeline.py:406-408) [diffusers absent: restated from memory].
@@ -30,33 +25,32 @@
 namespace {
 
 constexpr int TQ = 128;   // queries per CTA
-constexpr int TK = 128;   // keys per tile
+constexpr int TK = 64;    // keys per tile
+constexpr int ATTN_THREADS = 256 + 32;
 
 struct AttnParams {
     int Nq, Nk, d, heads;
-    int n_tiles;          // ceil(Nk / 128)
+    int n_tiles;          // ceil(Nk / TK)
     float c;              // scale * log2(e)
     __half* out;          // [B][Nq][C]
     long out_pitch;       // C
-    int causal;           // 1: key j is visible to query i only if j <= i (CLIP text encoder); short-key kernel only
-    int poly_exp;         // 1: half of the exponentials of the single-pass kernel on the FMA pipe (experiment, RF_ATTN_POLY=1)
+    int causal;           // 1: key j is visible to query i only if j <= i (CLIP text encoder)
 };
 
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t* v) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-          "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-        : "r"(taddr)
-        : "memory");
+__device__ __forceinline__ uint32_t pack_half2(float a, float b) {
+    const __half2 h = __floats2half2_rn(a, b);
+    return *reinterpret_cast<const uint32_t*>(&h);
 }
-__device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void named_bar_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
+__device__ __forceinline__ float ex2(float a) {
+    float r;
+    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(a));
+    return r;
+}
 
-// DPAD: head dim rounded up to 64 (Q/K slabs of 64 elements); NV: head dim rounded up to 16 (UMMA N of the PV product)
+// DPAD: head dim rounded up to 64 (Q / K slabs of 64 elements, the tail zero-filled by TMA); NV: head dim rounded up to
+// 16 (wgmma N of the P V product; V^T rows beyond d are zero-filled by TMA); NS: K / V^T ring depth
 template <int DPAD, int NV, int NS>
-__global__ void __launch_bounds__(320, 1)
+__global__ void __launch_bounds__(ATTN_THREADS, 1)
 k_flash_attn(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapK,
              const __grid_constant__ CUtensorMap mapVt, const AttnParams p) {
     extern __shared__ __align__(1024) uint8_t smem[];
@@ -64,24 +58,14 @@ k_flash_attn(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ C
     constexpr int NSLAB = DPAD / 64;
     constexpr int Q_BYTES = NSLAB * TQ * 128;
     constexpr int K_BYTES = NSLAB * TK * 128;
-    constexpr int V_SLAB = ((NV * 128 + 1023) / 1024) * 1024;   // one 64-key slab of V^T, padded to the swizzle atom
-    constexpr int V_BYTES = 2 * V_SLAB;
-    constexpr int P_BYTES = 2 * TQ * 128;                        // 128 x 128 fp16
+    constexpr int V_BYTES = ((NV * 128 + 1023) / 1024) * 1024;   // NV rows of 64 keys, padded to the swizzle atom
     uint8_t* sQ = smem;
     uint8_t* sK = sQ + Q_BYTES;                 // [NS][K_BYTES]
     uint8_t* sV = sK + NS * K_BYTES;            // [NS][V_BYTES]
-    uint8_t* sP = sV + NS * V_BYTES;            // [2][P_BYTES]
-    uint64_t* bars = reinterpret_cast<uint64_t*>(sP + 2 * P_BYTES);
+    uint64_t* bars = reinterpret_cast<uint64_t*>(sV + NS * V_BYTES);
     uint64_t* q_full = bars;                    // 1
     uint64_t* kv_full = bars + 1;               // NS
     uint64_t* kv_empty = kv_full + NS;          // NS
-    uint64_t* s_full = kv_empty + NS;           // 2
-    uint64_t* s_empty = s_full + 2;             // 2
-    uint64_t* p_full = s_empty + 2;             // 2
-    uint64_t* p_empty = p_full + 2;             // 2
-    uint64_t* o_full = p_empty + 2;             // 1
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(o_full + 1);
-    float* xchg = reinterpret_cast<float*>(tmem_slot + 2);   // [2][128] row max / row sum exchange between groups
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int q_blk = blockIdx.x, head = blockIdx.y, b = blockIdx.z;
@@ -91,870 +75,131 @@ k_flash_attn(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ C
         tc::mbar_init(q_full, 1);
         for (int i = 0; i < NS; ++i) {
             tc::mbar_init(&kv_full[i], 1);
-            tc::mbar_init(&kv_empty[i], 1);
+            tc::mbar_init(&kv_empty[i], 256);   // every consumer thread arrives once its P V has completed
         }
-        for (int i = 0; i < 2; ++i) {
-            tc::mbar_init(&s_full[i], 1);
-            tc::mbar_init(&s_empty[i], 128);
-            tc::mbar_init(&p_full[i], 128);
-            tc::mbar_init(&p_empty[i], 1);
-        }
-        tc::mbar_init(o_full, 1);
         tc::fence_barrier_init();
     }
-    if (warp == 1) {
-        tc::tmem_alloc(tmem_slot, 512);
-        tc::tmem_relinquish();
-    }
-    tc::fence_before_sync();
     __syncthreads();
-    tc::fence_after_sync();
-    const uint32_t tmem_base = *tmem_slot;
     rf_pdl_wait();         // prologue done; the producer grid must be complete before Q / K / V are read
-    const uint32_t tmem_O = tmem_base + 256;
 
-    if (warp == 0 && lane == 0) {
+    if (warp == 8) {
+        if (lane != 0) return;
         // ------------------------------------------------------------------ TMA producer
         tc::mbar_expect_tx(q_full, Q_BYTES);
 #pragma unroll
         for (int s = 0; s < NSLAB; ++s) tc::tma_load_4d(&mapQ, q_full, sQ + s * TQ * 128, s * 64, q_blk * TQ, head, b);
-        int it = 0;
-        for (int pass = 0; pass < 2; ++pass)
-            for (int j = 0; j < T; ++j, ++it) {
-                const int st = it % NS;
-                tc::mbar_wait(&kv_empty[st], ((it / NS) & 1) ^ 1);
-                tc::mbar_expect_tx(&kv_full[st], K_BYTES + (pass ? 2 * NV * 128 : 0));
-#pragma unroll
-                for (int s = 0; s < NSLAB; ++s)
-                    tc::tma_load_4d(&mapK, &kv_full[st], sK + st * K_BYTES + s * TK * 128, s * 64, j * TK, head, b);
-                if (pass) {
-                    tc::tma_load_4d(&mapVt, &kv_full[st], sV + st * V_BYTES, j * TK, 0, head, b);
-                    tc::tma_load_4d(&mapVt, &kv_full[st], sV + st * V_BYTES + V_SLAB, j * TK + 64, 0, head, b);
-                }
-            }
-    } else if (warp == 1 && lane == 0) {
-        // ------------------------------------------------------------------ MMA issuer
-        constexpr uint32_t idesc_qk = tc::make_idesc_f16(TQ, TK);
-        constexpr uint32_t idesc_pv = tc::make_idesc_f16(TQ, NV);
-        tc::mbar_wait(q_full, 0);
-        tc::fence_after_sync();
-        const uint32_t q_base = tc::smem_u32(sQ);
-        auto issue_qk = [&](int it, int j) {     // S_{j&1} = Q K_j^T
-            const int st = it % NS;
-            tc::mbar_wait(&kv_full[st], (it / NS) & 1);
-            tc::fence_after_sync();
-            const uint32_t k_base = tc::smem_u32(sK + st * K_BYTES);
-#pragma unroll
-            for (int s = 0; s < NSLAB; ++s)
-#pragma unroll
-                for (int k = 0; k < 4; ++k)
-                    tc::mma_f16(tmem_base + (j & 1) * 128, tc::make_desc_sw128(q_base + s * TQ * 128 + k * 32),
-                                tc::make_desc_sw128(k_base + s * TK * 128 + k * 32), idesc_qk, (s | k) ? 1u : 0u);
-            tc::mma_commit(&s_full[j & 1]);
-        };
-        int se_cnt[2] = {0, 0};                  // completed uses of each S buffer (for s_empty parity)
-        // ---- pass 1: scores only
         for (int j = 0; j < T; ++j) {
-            const int i = j & 1;
-            if (se_cnt[i] > 0) {
-                tc::mbar_wait(&s_empty[i], (se_cnt[i] - 1) & 1);
-                tc::fence_after_sync();
-            }
-            issue_qk(j, j);
-            ++se_cnt[i];
-            tc::mma_commit(&kv_empty[j % NS]);   // K_j is free once this QK^T has completed
-        }
-        // ---- pass 2: scores, then P V
-        int pe_cnt[2] = {0, 0};
-        auto qk2 = [&](int j) {
-            const int i = j & 1;
-            if (se_cnt[i] > 0) {
-                tc::mbar_wait(&s_empty[i], (se_cnt[i] - 1) & 1);
-                tc::fence_after_sync();
-            }
-            issue_qk(T + j, j);
-            ++se_cnt[i];
-        };
-        // look-ahead: with >= 2 K/V stages the next two score tiles are issued before the first P V (ping-pong on the
-        // two S buffers); with a single stage the stage is only released by the P V that consumed it
-        constexpr int LA = NS >= 2 ? 2 : 1;
-        for (int j = 0; j < LA && j < T; ++j) qk2(j);
-        for (int j = 0; j < T; ++j) {
-            const int i = j & 1;
-            const int it = T + j, st = it % NS;
-            tc::mbar_wait(&p_full[i], pe_cnt[i] & 1);
-            tc::fence_after_sync();
-            const uint32_t p_base = tc::smem_u32(sP + i * P_BYTES);
-            const uint32_t v_base = tc::smem_u32(sV + st * V_BYTES);
-#pragma unroll
-            for (int s = 0; s < 2; ++s)
-#pragma unroll
-                for (int k = 0; k < 4; ++k)
-                    tc::mma_f16(tmem_O, tc::make_desc_sw128(p_base + s * TQ * 128 + k * 32),
-                                tc::make_desc_sw128(v_base + s * V_SLAB + k * 32), idesc_pv, (j | s | k) ? 1u : 0u);
-            tc::mma_commit(&p_empty[i]);
-            tc::mma_commit(&kv_empty[st]);       // K_j and V_j free once P V (and the earlier QK^T) have completed
-            ++pe_cnt[i];
-            if (j + LA < T) qk2(j + LA);
-        }
-        tc::mma_commit(o_full);
-    } else if (warp >= 2) {
-        // ------------------------------------------------------------------ softmax groups
-        const int g = (warp - 2) >> 2;           // 0: even tiles, 1: odd tiles
-        const int q = warp & 3;                  // TMEM lane quarter
-        const int row = q * 32 + lane;
-        const uint32_t t_row = tmem_base + (static_cast<uint32_t>(q * 32) << 16);
-        int sf_phase = 0;
-        float m = -INFINITY;
-        // ---- pass 1: row maximum of the raw scores over this group's tiles
-        for (int j = g; j < T; j += 2) {
-            tc::mbar_wait(&s_full[g], sf_phase);
-            sf_phase ^= 1;
-            tc::fence_after_sync();
-            const int kmax = p.Nk - j * TK;      // valid keys in this tile
-#pragma unroll 1
-            for (int c0 = 0; c0 < TK; c0 += 32) {
-                uint32_t v[32];
-                tc::tmem_ld_32x32(t_row + g * 128 + c0, v);
-                tc::tmem_wait_ld();
-#pragma unroll
-                for (int i = 0; i < 32; ++i)
-                    if (c0 + i < kmax) m = fmaxf(m, __uint_as_float(v[i]));
-            }
-            tc::fence_before_sync();
-            tc::mbar_arrive(&s_empty[g]);
-        }
-        xchg[g * 128 + row] = m;
-        named_bar_sync(1, 256);
-        m = fmaxf(xchg[row], xchg[128 + row]);
-        const float mc = m * p.c;
-        named_bar_sync(1, 256);                  // everyone has read the maxima before xchg is reused for the sums
-        // ---- pass 2: P = exp2(S*c - m*c), row sums, P -> shared memory (K-major, 128-byte swizzle)
-        float l = 0.f;
-        int pe_phase = 0, n_mine = 0;
-        uint8_t* myP = sP + g * P_BYTES;
-        for (int j = g; j < T; j += 2, ++n_mine) {
-            tc::mbar_wait(&s_full[g], sf_phase);
-            sf_phase ^= 1;
-            tc::fence_after_sync();
-            if (n_mine > 0) {                    // the previous P V that read this P buffer must have completed
-                tc::mbar_wait(&p_empty[g], pe_phase);
-                pe_phase ^= 1;
-            }
-            const int kmax = p.Nk - j * TK;
-#pragma unroll 1
-            for (int c0 = 0; c0 < TK; c0 += 32) {
-                uint32_t v[32];
-                tc::tmem_ld_32x32(t_row + g * 128 + c0, v);
-                tc::tmem_wait_ld();
-                uint32_t pk[16];
-#pragma unroll
-                for (int i = 0; i < 32; i += 2) {
-                    // two exponentials per MUFU op (ex2.approx.f16x2): the SFU, not the tensor pipe, bounds small
-                    // head dims.  The argument is formed in fp32 and rounded once to fp16; P is stored as fp16 anyway.
-                    const float a0 = (c0 + i < kmax) ? fmaf(__uint_as_float(v[i]), p.c, -mc) : -INFINITY;
-                    const float a1 = (c0 + i + 1 < kmax) ? fmaf(__uint_as_float(v[i + 1]), p.c, -mc) : -INFINITY;
-                    const __half2 arg = __floats2half2_rn(a0, a1);
-                    uint32_t hbits;
-                    asm("ex2.approx.f16x2 %0, %1;" : "=r"(hbits) : "r"(*reinterpret_cast<const uint32_t*>(&arg)));
-                    const __half2 h = *reinterpret_cast<const __half2*>(&hbits);
-                    // accumulate the row sum from the rounded values the P V product will actually use
-                    const float2 hr = __half22float2(h);
-                    l += hr.x + hr.y;
-                    pk[i >> 1] = hbits;
-                }
-                // columns c0..c0+31 = 4 chunks of 8 halves; slab = c0 / 64, chunk index within the 128-byte row
-                const int slab = c0 >> 6;
-#pragma unroll
-                for (int ch = 0; ch < 4; ++ch) {
-                    const int chunk = ((c0 & 63) >> 3) + ch;
-                    uint4 val = make_uint4(pk[4 * ch], pk[4 * ch + 1], pk[4 * ch + 2], pk[4 * ch + 3]);
-                    *reinterpret_cast<uint4*>(myP + slab * TQ * 128 + row * 128 + ((chunk ^ (row & 7)) << 4)) = val;
-                }
-            }
-            tc::fence_before_sync();
-            tc::mbar_arrive(&s_empty[g]);        // S buffer may be overwritten by the next QK^T
-            fence_async_smem();                  // make the P stores visible to the tensor-core (async) proxy
-            tc::mbar_arrive(&p_full[g]);
-        }
-        xchg[g * 128 + row] = l;
-        named_bar_sync(1, 256);
-        if (g == 0) {
-            // ---- epilogue (group A): O / rowsum -> fp16
-            const float inv = 1.f / (xchg[row] + xchg[128 + row]);
-            tc::mbar_wait(o_full, 0);
-            tc::fence_after_sync();
-            const int qi = q_blk * TQ + row;
-            __half* dst = p.out + (static_cast<long>(b) * p.Nq + qi) * p.out_pitch + head * p.d;
-#pragma unroll 1
-            for (int c0 = 0; c0 < NV; c0 += 16) {
-                uint32_t v[16];
-                tmem_ld16(t_row + 256 + c0, v);
-                tc::tmem_wait_ld();
-                if (qi < p.Nq) {
-#pragma unroll
-                    for (int ch = 0; ch < 2; ++ch) {
-                        const int col = c0 + 8 * ch;
-                        if (col < p.d) {         // d is a multiple of 8
-                            __half2 h0 = __floats2half2_rn(__uint_as_float(v[8 * ch + 0]) * inv, __uint_as_float(v[8 * ch + 1]) * inv);
-                            __half2 h1 = __floats2half2_rn(__uint_as_float(v[8 * ch + 2]) * inv, __uint_as_float(v[8 * ch + 3]) * inv);
-                            __half2 h2 = __floats2half2_rn(__uint_as_float(v[8 * ch + 4]) * inv, __uint_as_float(v[8 * ch + 5]) * inv);
-                            __half2 h3 = __floats2half2_rn(__uint_as_float(v[8 * ch + 6]) * inv, __uint_as_float(v[8 * ch + 7]) * inv);
-                            uint4 pk;
-                            pk.x = *reinterpret_cast<uint32_t*>(&h0);
-                            pk.y = *reinterpret_cast<uint32_t*>(&h1);
-                            pk.z = *reinterpret_cast<uint32_t*>(&h2);
-                            pk.w = *reinterpret_cast<uint32_t*>(&h3);
-                            *reinterpret_cast<uint4*>(dst + col) = pk;
-                        }
-                    }
-                }
-            }
-            tc::fence_before_sync();
-        }
-    }
-    __syncthreads();
-    if (warp == 1) {
-        tc::fence_after_sync();
-        tc::tmem_dealloc(tmem_base, 512);
-    }
-}
-
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t* v) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-        "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};"
-        :
-        : "r"(taddr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]),
-          "r"(v[9]), "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15])
-        : "memory");
-}
-__device__ __forceinline__ void tmem_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// ------------------------------------------------------------------------------------------------------------------
-// Single-pass variant (head dims up to 112): every key tile is visited once.
-//   * The two softmax groups still take alternate key tiles of the same 128 queries, but each group keeps its OWN
-//     reference maximum and its OWN accumulator O_g in TMEM, so the groups never exchange anything inside the loop;
-//     the epilogue merges  O = (O_A 2^(mA-m) + O_B 2^(mB-m)) / (l_A 2^(mA-m) + l_B 2^(mB-m)).
-//   * The reference maximum is only raised when a tile exceeds it by more than 2^RESCALE_LOG2 (probabilities stay
-//     <= 2^RESCALE_LOG2, safe in fp16); raising it rescales O_g in TMEM (tcgen05.ld -> multiply -> tcgen05.st), which
-//     happens a handful of times per row instead of once per tile.
-//   * Row sums come out of the tensor core: the V^T tiles carry 16 extra rows of ones below the head dim, so column NV
-//     of O_g is sum_j P_ij of exactly the fp16 values the P V product used.
-//   * A group pulls its whole 128-score row into registers and frees the S buffer before it evaluates the
-//     exponentials, so the next Q K^T overlaps the softmax arithmetic.
-// TMEM: S0 | S1 | O_A (NV+16 columns) | O_B (NV+16 columns).
-constexpr float RESCALE_LOG2 = 4.f;
-
-// NG softmax groups (2 or 4) take the key tiles round-robin; a tile is TKT = 256/NG keys, so the NG score buffers always
-// fill TMEM columns [0, 256) and O_g sits at 256 + g*(NV+16).  NG = 4 (head dim <= 48) puts four independent warps on
-// every SM sub-partition: while one waits for its scores or drains TMEM (tcgen05.ld, 64 B/clk per SM), the others keep
-// the MUFU pipe busy — with NG = 2 each sub-partition has only two warps and the phases of a warp run back to back.
-template <int DPAD, int NV, int NKS, int NVS, int NG>
-__global__ void __launch_bounds__(96 + 128 * NG, 1)
-k_flash_attn1(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapK,
-              const __grid_constant__ CUtensorMap mapVt, const AttnParams p) {
-    extern __shared__ __align__(1024) uint8_t smem[];
-    rf_pdl_trigger();      // PDL (rf_common.h): dependents may start their prologue
-    constexpr int TKT = 256 / NG;                                 // keys per tile
-    constexpr int KSL = TKT / 64;                                 // 64-key slabs per tile (P and V^T)
-    constexpr int NSLAB = DPAD / 64;
-    constexpr int NVP = NV + 16;                                  // head dim columns + the row-sum column block
-    static_assert(NG == 2 || NG == 4, "two or four softmax groups");
-    static_assert(256 + NG * NVP <= 512, "TMEM budget");
-    constexpr int Q_BYTES = NSLAB * TQ * 128;
-    constexpr int K_BYTES = NSLAB * TKT * 128;
-    constexpr int V_SLAB = ((NVP * 128 + 1023) / 1024) * 1024;
-    constexpr int V_BYTES = KSL * V_SLAB;
-    constexpr int P_BYTES = KSL * TQ * 128;
-    uint8_t* sQ = smem;
-    uint8_t* sK = sQ + Q_BYTES;                 // [NKS][K_BYTES]  K tiles are released by their Q K^T (early)
-    uint8_t* sV = sK + NKS * K_BYTES;           // [NVS][V_BYTES]  V^T tiles by their P V (late): separate rings
-    uint8_t* sP = sV + NVS * V_BYTES;           // [NG][P_BYTES]
-    uint64_t* bars = reinterpret_cast<uint64_t*>(sP + NG * P_BYTES);
-    uint64_t* q_full = bars;
-    uint64_t* k_full = bars + 1;
-    uint64_t* k_empty = k_full + NKS;
-    uint64_t* v_full = k_empty + NKS;
-    uint64_t* v_empty = v_full + NVS;
-    uint64_t* s_full = v_empty + NVS;
-    uint64_t* s_empty = s_full + NG;
-    uint64_t* p_full = s_empty + NG;
-    uint64_t* p_empty = p_full + NG;
-    uint64_t* o_full = p_empty + NG;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(o_full + 1);
-    float* xchg = reinterpret_cast<float*>(tmem_slot + 2);       // [NG][128] reference maxima of the groups
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int q_blk = blockIdx.x, head = blockIdx.y, b = blockIdx.z;
-    const int T = p.n_tiles;
-
-    if (threadIdx.x == 0) {
-        tc::mbar_init(q_full, 1);
-        for (int i = 0; i < NKS; ++i) {
-            tc::mbar_init(&k_full[i], 1);
-            tc::mbar_init(&k_empty[i], 1);
-        }
-        for (int i = 0; i < NVS; ++i) {
-            tc::mbar_init(&v_full[i], 1);
-            tc::mbar_init(&v_empty[i], 1);
-        }
-        for (int i = 0; i < NG; ++i) {
-            tc::mbar_init(&s_full[i], 1);
-            tc::mbar_init(&s_empty[i], 128);
-            tc::mbar_init(&p_full[i], 128);
-            tc::mbar_init(&p_empty[i], 1);
-        }
-        tc::mbar_init(o_full, 1);
-        tc::fence_barrier_init();
-    }
-    if (warp == 1) {
-        tc::tmem_alloc(tmem_slot, 512);
-        tc::tmem_relinquish();
-    }
-    // rows NV .. NV+15 of every V^T slab = 1.0 (never touched by the TMA boxes, which are NV rows tall)
-    for (int i = threadIdx.x; i < NVS * KSL * 16 * 8; i += blockDim.x) {
-        const int ch = i & 7, r = (i >> 3) & 15, sl = (i >> 7) % KSL, st = (i >> 7) / KSL;
-        *reinterpret_cast<uint4*>(sV + st * V_BYTES + sl * V_SLAB + (NV + r) * 128 + ch * 16) =
-            make_uint4(0x3C003C00u, 0x3C003C00u, 0x3C003C00u, 0x3C003C00u);
-    }
-    fence_async_smem();
-    tc::fence_before_sync();
-    __syncthreads();
-    tc::fence_after_sync();
-    const uint32_t tmem_base = *tmem_slot;
-    rf_pdl_wait();         // prologue done; the producer grid must be complete before Q / K / V are read
-    const uint32_t tmem_O = tmem_base + 256;
-
-    if (warp == 0 && lane == 0) {
-        // ------------------------------------------------------------------ TMA producer
-        tc::mbar_expect_tx(q_full, Q_BYTES);
-#pragma unroll
-        for (int s = 0; s < NSLAB; ++s) tc::tma_load_4d(&mapQ, q_full, sQ + s * TQ * 128, s * 64, q_blk * TQ, head, b);
-        // K runs NG tiles ahead of V^T: the next Q K^T of a group is issued while its softmax is still running
-        auto load_k = [&](int j) {
-            const int st = j % NKS;
-            tc::mbar_wait(&k_empty[st], ((j / NKS) & 1) ^ 1);
-            tc::mbar_expect_tx(&k_full[st], K_BYTES);
+            const int st = j % NS;
+            tc::mbar_wait(&kv_empty[st], ((j / NS) & 1) ^ 1);
+            tc::mbar_expect_tx(&kv_full[st], K_BYTES + NV * 128);
 #pragma unroll
             for (int s = 0; s < NSLAB; ++s)
-                tc::tma_load_4d(&mapK, &k_full[st], sK + st * K_BYTES + s * TKT * 128, s * 64, j * TKT, head, b);
-        };
-        for (int j = 0; j < NG && j < T; ++j) load_k(j);
-        for (int j = 0; j < T; ++j) {
-            if (j + NG < T) load_k(j + NG);
-            const int st = j % NVS;
-            tc::mbar_wait(&v_empty[st], ((j / NVS) & 1) ^ 1);
-            tc::mbar_expect_tx(&v_full[st], KSL * NV * 128);
-#pragma unroll
-            for (int s = 0; s < KSL; ++s)
-                tc::tma_load_4d(&mapVt, &v_full[st], sV + st * V_BYTES + s * V_SLAB, j * TKT + 64 * s, 0, head, b);
+                tc::tma_load_4d(&mapK, &kv_full[st], sK + st * K_BYTES + s * TK * 128, s * 64, j * TK, head, b);
+            tc::tma_load_4d(&mapVt, &kv_full[st], sV + st * V_BYTES, j * TK, 0, head, b);
         }
-    } else if (warp == 1 && lane == 0) {
-        // ------------------------------------------------------------------ Q K^T issuer
-        // Two issuing threads (this one and the P V issuer in the last warp): a single thread spends ~1000 cycles per
-        // 128-key tile on descriptors, polling and commits for the 12 MMAs, which is the whole MUFU budget of the tile.
-        // Both are event driven: they poll, per softmax group, whether that group's next MMA can go and issue whatever
-        // is ready, so no group ever waits for another group's exponentials.
-        constexpr uint32_t idesc_qk = tc::make_idesc_f16(TQ, TKT);
-        tc::mbar_wait(q_full, 0);
-        tc::fence_after_sync();
-        const uint32_t q_lo = tc::desc_lo_sw128(tc::smem_u32(sQ));
-        int qk_next[NG], se_cnt[NG];
-#pragma unroll
-        for (int i = 0; i < NG; ++i) {
-            qk_next[i] = i;
-            se_cnt[i] = 0;
-        }
-        // K tiles arrive in tile order through a ring: a tile may only be issued while it is less than a ring depth
-        // ahead of the oldest tile not yet issued (whose completion frees the next slot)
-        for (;;) {
-            int qk_min = T;
-#pragma unroll
-            for (int i = 0; i < NG; ++i) qk_min = min(qk_min, qk_next[i]);
-            if (qk_min >= T) break;
-            bool any = false;
-#pragma unroll
-            for (int i = 0; i < NG; ++i) {
-                const int j = qk_next[i];
-                if (j >= T || j - qk_min >= NKS) continue;
-                const int st = j % NKS;
-                if (se_cnt[i] > 0 && !tc::mbar_test(&s_empty[i], (se_cnt[i] - 1) & 1)) continue;   // scores still being read
-                if (!tc::mbar_test(&k_full[st], (j / NKS) & 1)) continue;
-                tc::fence_after_sync();
-                const uint32_t k_lo = tc::desc_lo_sw128(tc::smem_u32(sK + st * K_BYTES));
-#pragma unroll
-                for (int s = 0; s < NSLAB; ++s)
-#pragma unroll
-                    for (int k = 0; k < 4; ++k)
-                        tc::mma_f16_lo(tmem_base + i * TKT, q_lo + ((s * TQ * 128 + k * 32) >> 4),
-                                       k_lo + ((s * TKT * 128 + k * 32) >> 4), idesc_qk, (s | k) ? 1u : 0u);
-                tc::mma_commit(&s_full[i]);
-                tc::mma_commit(&k_empty[st]);
-                ++se_cnt[i];
-                qk_next[i] = j + NG;
-                any = true;
-            }
-            if (!any) __nanosleep(20);
-        }
-    } else if (warp == 2 + 4 * NG && lane == 0) {
-        // ------------------------------------------------------------------ P V issuer
-        constexpr uint32_t idesc_pv = tc::make_idesc_f16(TQ, NVP);
-        int pv_next[NG], pe_cnt[NG];
-#pragma unroll
-        for (int i = 0; i < NG; ++i) {
-            pv_next[i] = i;
-            pe_cnt[i] = 0;
-        }
-        for (;;) {
-            int pv_min = T;
-#pragma unroll
-            for (int i = 0; i < NG; ++i) pv_min = min(pv_min, pv_next[i]);
-            if (pv_min >= T) break;
-            bool any = false;
-#pragma unroll
-            for (int i = 0; i < NG; ++i) {
-                const int j = pv_next[i];
-                if (j >= T || j - pv_min >= NVS) continue;
-                const int st = j % NVS;
-                if (!tc::mbar_test(&p_full[i], pe_cnt[i] & 1)) continue;
-                if (!tc::mbar_test(&v_full[st], (j / NVS) & 1)) continue;
-                tc::fence_after_sync();
-                const uint32_t p_lo = tc::desc_lo_sw128(tc::smem_u32(sP + i * P_BYTES));
-                const uint32_t v_lo = tc::desc_lo_sw128(tc::smem_u32(sV + st * V_BYTES));
-#pragma unroll
-                for (int s = 0; s < KSL; ++s)
-#pragma unroll
-                    for (int k = 0; k < 4; ++k)
-                        tc::mma_f16_lo(tmem_O + i * NVP, p_lo + ((s * TQ * 128 + k * 32) >> 4),
-                                       v_lo + ((s * V_SLAB + k * 32) >> 4), idesc_pv, ((j >= NG) | s | k) ? 1u : 0u);
-                tc::mma_commit(&p_empty[i]);
-                tc::mma_commit(&v_empty[st]);
-                ++pe_cnt[i];
-                pv_next[i] = j + NG;
-                any = true;
-            }
-            if (!any) __nanosleep(20);
-        }
-        tc::mma_commit(o_full);
-    } else if (warp >= 2 && warp < 2 + 4 * NG) {
-        // ------------------------------------------------------------------ softmax groups
-        const int g = (warp - 2) >> 2;
-        const int q = warp & 3;
-        const int row = q * 32 + lane;
-        const uint32_t t_row = tmem_base + (static_cast<uint32_t>(q * 32) << 16);
-        const uint32_t t_Og = t_row + 256 + g * NVP;
-        const float c = p.c;
-        int sf_phase = 0, pe_phase = 0, n_mine = 0;
-        float m_ref = -INFINITY;                 // reference maximum (raw score units) of this group
-        uint8_t* myP = sP + g * P_BYTES;
-        for (int j = g; j < T; j += NG, ++n_mine) {
-            tc::mbar_wait(&s_full[g], sf_phase);
-            sf_phase ^= 1;
-            tc::fence_after_sync();
-            uint32_t v[TKT];
-#pragma unroll
-            for (int c0 = 0; c0 < TKT; c0 += 32) tc::tmem_ld_32x32(t_row + g * TKT + c0, v + c0);
-            tc::tmem_wait_ld();
-            tc::fence_before_sync();
-            tc::mbar_arrive(&s_empty[g]);        // the scores are in registers: the next Q K^T may overwrite S
-            const int kmax = p.Nk - j * TKT;
-            if (kmax < TKT) {
-#pragma unroll
-                for (int i = 0; i < TKT; ++i)
-                    if (i >= kmax) v[i] = 0xff800000u;   // -inf
-            }
-            float mx[8];                          // eight independent chains: the maximum is latency, not issue, bound
-#pragma unroll
-            for (int i = 0; i < 8; ++i) mx[i] = __uint_as_float(v[i]);
-#pragma unroll
-            for (int i = 8; i < TKT; i += 16)
-#pragma unroll
-                for (int e = 0; e < 8; ++e)
-                    mx[e] = fmaxf(mx[e], fmaxf(__uint_as_float(v[i + e]), i + 8 + e < TKT ? __uint_as_float(v[i + 8 + e]) : -INFINITY));
-            const float mt = fmaxf(fmaxf(fmaxf(mx[0], mx[1]), fmaxf(mx[2], mx[3])), fmaxf(fmaxf(mx[4], mx[5]), fmaxf(mx[6], mx[7])));
-            const bool grow = (mt - m_ref) * c > RESCALE_LOG2;   // always true on the first tile (m_ref = -inf)
-            float fac = 1.f;
-            if (grow) {
-                fac = exp2f((m_ref - mt) * c);                   // 0 on the first tile
-                m_ref = mt;
-            }
-            if (n_mine > 0) {
-                tc::mbar_wait(&p_empty[g], pe_phase);            // previous P V of this group done: P buffer free, O_g quiet
-                pe_phase ^= 1;
-                tc::fence_after_sync();
-                if (__any_sync(0xffffffffu, grow)) {
-#pragma unroll 1
-                    for (int c0 = 0; c0 < NVP; c0 += 16) {
-                        uint32_t o[16];
-                        tmem_ld16(t_Og + c0, o);
-                        tc::tmem_wait_ld();
-#pragma unroll
-                        for (int i = 0; i < 16; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * fac);
-                        tmem_st16(t_Og + c0, o);
-                    }
-                    tmem_wait_st();
-                }
-            }
-            const float mc = m_ref * c;
-#pragma unroll
-            for (int c0 = 0; c0 < TKT; c0 += 8) {
-                uint32_t pk[4];
-                if (p.poly_exp && (c0 & 8)) {
-                    // every second group of 8 keys: 2^a on the FMA / ALU pipes instead of MUFU (the exponentials of a key
-                    // tile are the whole MUFU budget of that tile): n = round(a) by the magic-number add, 2^(a - n) by a
-                    // degree-3 polynomial on [-0.5, 0.5] (7.5e-5 relative, below the 4.9e-4 fp16 rounding of P), exponent
-                    // bits of n added to the result.  a <= RESCALE_LOG2; a < -24 is clamped (2^-24 = fp16's smallest).
-#pragma unroll
-                    for (int i = 0; i < 8; i += 2) {
-                        float e[2];
-#pragma unroll
-                        for (int u = 0; u < 2; ++u) {
-                            const float a = fmaxf(fmaf(__uint_as_float(v[c0 + i + u]), c, -mc), -24.f);
-                            const float t = a + 12582912.f;
-                            const float f = a - (t - 12582912.f);
-                            const float q = fmaf(fmaf(fmaf(0.05517144f, f, 0.24261071f), f, 0.69326097f), f, 0.99992812f);
-                            e[u] = __int_as_float(__float_as_int(q) + (__float_as_int(t) << 23));
-                        }
-                        const __half2 h = __floats2half2_rn(e[0], e[1]);
-                        pk[i >> 1] = *reinterpret_cast<const uint32_t*>(&h);
-                    }
-                } else
-#pragma unroll
-                for (int i = 0; i < 8; i += 2) {
-                    // the argument (<= RESCALE_LOG2) is formed in fp32 and rounded once to fp16; P is fp16 anyway
-                    const float a0 = fmaf(__uint_as_float(v[c0 + i]), c, -mc);
-                    const float a1 = fmaf(__uint_as_float(v[c0 + i + 1]), c, -mc);
-#ifdef RF_ATTN_EXP_F16X2
-                    const __half2 arg = __floats2half2_rn(a0, a1);
-                    asm("ex2.approx.f16x2 %0, %1;" : "=r"(pk[i >> 1]) : "r"(*reinterpret_cast<const uint32_t*>(&arg)));
-#else
-                    float e0, e1;
-                    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e0) : "f"(a0));
-                    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e1) : "f"(a1));
-                    const __half2 h = __floats2half2_rn(e0, e1);
-                    pk[i >> 1] = *reinterpret_cast<const uint32_t*>(&h);
-#endif
-                }
-                const int slab = c0 >> 6, chunk = (c0 & 63) >> 3;
-                *reinterpret_cast<uint4*>(myP + slab * TQ * 128 + row * 128 + ((chunk ^ (row & 7)) << 4)) =
-                    make_uint4(pk[0], pk[1], pk[2], pk[3]);
-            }
-            fence_async_smem();                  // P stores -> async proxy
-            tc::fence_before_sync();             // orders the tcgen05.st of a rescale before the P V issued after p_full
-            tc::mbar_arrive(&p_full[g]);
-        }
-        // ---- epilogue: merge the groups' accumulators
-        xchg[g * 128 + row] = m_ref;             // -inf for a group that saw no tile
-        named_bar_sync(1, 128 * NG);
-        float mg[NG], fg[NG];
-        float mm = -INFINITY;
-#pragma unroll
-        for (int i = 0; i < NG; ++i) {
-            mg[i] = i < T ? xchg[i * 128 + row] : -INFINITY;
-            mm = fmaxf(mm, mg[i]);
-        }
-#pragma unroll
-        for (int i = 0; i < NG; ++i) fg[i] = i < T ? exp2f((mg[i] - mm) * c) : 0.f;
-        tc::mbar_wait(o_full, 0);
-        tc::fence_after_sync();
-        float lsum = 0.f;
-#pragma unroll
-        for (int i = 0; i < NG; ++i) {
-            if (i < T) {                          // accumulators of groups without a tile were never written
-                uint32_t l16[16];
-                tmem_ld16(t_row + 256 + i * NVP + NV, l16);
-                tc::tmem_wait_ld();
-                lsum = fmaf(__uint_as_float(l16[0]), fg[i], lsum);
-            }
-        }
-        const float inv = 1.f / lsum;
-        const int qi = q_blk * TQ + row;
-        __half* dst = p.out + (static_cast<long>(b) * p.Nq + qi) * p.out_pitch + head * p.d;
-#pragma unroll 1
-        for (int c0 = g * 16; c0 < NV; c0 += 16 * NG) {   // the groups take the 16-column chunks round-robin
-            float acc[16];
-#pragma unroll
-            for (int e = 0; e < 16; ++e) acc[e] = 0.f;
-#pragma unroll
-            for (int i = 0; i < NG; ++i) {
-                if (i < T) {
-                    uint32_t o[16];
-                    tmem_ld16(t_row + 256 + i * NVP + c0, o);
-                    tc::tmem_wait_ld();
-                    const float w = fg[i] * inv;
-#pragma unroll
-                    for (int e = 0; e < 16; ++e) acc[e] = fmaf(__uint_as_float(o[e]), w, acc[e]);
-                }
-            }
-            if (qi < p.Nq) {
-#pragma unroll
-                for (int ch = 0; ch < 2; ++ch) {
-                    const int col = c0 + 8 * ch;
-                    if (col < p.d) {             // d is a multiple of 8
-                        uint32_t pk[4];
-#pragma unroll
-                        for (int e = 0; e < 4; ++e) {
-                            const __half2 h = __floats2half2_rn(acc[8 * ch + 2 * e], acc[8 * ch + 2 * e + 1]);
-                            pk[e] = *reinterpret_cast<const uint32_t*>(&h);
-                        }
-                        *reinterpret_cast<uint4*>(dst + col) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-                    }
-                }
-            }
-        }
-        tc::fence_before_sync();
+        return;
     }
-    __syncthreads();
-    if (warp == 1) {
-        tc::fence_after_sync();
-        tc::tmem_dealloc(tmem_base, 512);
-    }
-}
 
-// ------------------------------------------------------------------------------------------------------------------
-// Short key sequences (Nk <= 128: the cross-attention to the 77 text tokens).  One key tile, so no online softmax; what
-// dominates the streaming kernel here is its fixed cost per CTA (TMEM allocation, barrier setup, a dependent chain of
-// TMA -> MMA -> tcgen05.ld -> MMA latencies: 5.4 us for 128 queries).  This kernel is persistent instead: a CTA takes a
-// contiguous range of (image, head, query block) items, keeps K / V^T of the current head in shared memory, and
-// software-pipelines the items over two Q / S / P / O buffers:
-//   control thread (warp 0): TMA of Q_{n+1}, K/V^T on a head change; issues Q_n K^T before it waits for P_{n-1}, then P_{n-1} V
-//   warps 1-4 (one query row per thread): scores_n -> max -> exp2 -> P_n ; then the epilogue of item n-1 (O / l -> fp16)
-// Row sums again come from 16 rows of ones under V^T.  TMEM: S0 | S1 | O0 | O1.
-template <int DPAD, int NV>
-__global__ void __launch_bounds__(160, 1)
-k_attn_short(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapK,
-             const __grid_constant__ CUtensorMap mapVt, const AttnParams p, int n_items, int nqb) {
-    extern __shared__ __align__(1024) uint8_t smem[];
-    rf_pdl_trigger();      // PDL (rf_common.h): dependents may start their prologue
-    constexpr int NSLAB = DPAD / 64;
-    constexpr int NVP = NV + 16;
-    static_assert(256 + 2 * NVP <= 512, "TMEM budget");
-    constexpr int Q_BYTES = NSLAB * TQ * 128;
-    constexpr int K_BYTES = NSLAB * TK * 128;
-    constexpr int V_SLAB = ((NVP * 128 + 1023) / 1024) * 1024;
-    constexpr int V_BYTES = 2 * V_SLAB;
-    constexpr int P_BYTES = 2 * TQ * 128;
-    uint8_t* sQ = smem;                         // [2][Q_BYTES]
-    uint8_t* sK = sQ + 2 * Q_BYTES;
-    uint8_t* sV = sK + K_BYTES;
-    uint8_t* sP = sV + V_BYTES;                 // [2][P_BYTES]
-    uint64_t* bars = reinterpret_cast<uint64_t*>(sP + 2 * P_BYTES);
-    uint64_t* q_full = bars;                    // [2]
-    uint64_t* q_empty = bars + 2;               // [2]
-    uint64_t* kv_full = bars + 4;               // 1
-    uint64_t* s_full = bars + 5;                // [2]
-    uint64_t* s_empty = bars + 7;               // [2]
-    uint64_t* p_full = bars + 9;                // [2]
-    uint64_t* o_full = bars + 11;               // [2]
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 13);
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int per = (n_items + gridDim.x - 1) / gridDim.x;
-    const int w0 = blockIdx.x * per, w1 = min(n_items, w0 + per);
-    const int ncols = ((p.Nk + 31) / 32) * 32;  // score columns actually read back
-
-    if (threadIdx.x == 0) {
-        for (int i = 0; i < 2; ++i) {
-            tc::mbar_init(&q_full[i], 1);
-            tc::mbar_init(&q_empty[i], 1);
-            tc::mbar_init(&s_full[i], 1);
-            tc::mbar_init(&s_empty[i], 128);
-            tc::mbar_init(&p_full[i], 128);
-            tc::mbar_init(&o_full[i], 1);
+    // ---------------------------------------------------------------------- consumers
+    const int wg = warp >> 2;
+    const int frag_row = wg * 64 + (warp & 3) * 16 + (lane >> 2), frag_col = 2 * (lane & 3);
+    const int q0 = q_blk * TQ + frag_row, q1 = q0 + 8;       // the two query rows of this thread
+    const float c = p.c;
+    float o[NV / 2];
+#pragma unroll
+    for (int i = 0; i < NV / 2; ++i) o[i] = 0.f;
+    float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;   // running maxima (raw score units) and row sums
+    const uint32_t q_base = tc::smem_u32(sQ) + wg * (64 * 128);
+    tc::mbar_wait(q_full, 0);
+    for (int j = 0; j < T; ++j) {
+        const int st = j % NS;
+        tc::mbar_wait(&kv_full[st], (j / NS) & 1);
+        // ---- S = Q K_j^T
+        float s[TK / 2];
+        const uint32_t k_base = tc::smem_u32(sK + st * K_BYTES);
+        tc::wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < DPAD / 16; ++kk) {
+            const int sl = kk >> 2, k = kk & 3;
+            tc::wgmma_ss<TK>(s, tc::make_desc_sw128(q_base + sl * TQ * 128 + k * 32),
+                             tc::make_desc_sw128(k_base + sl * TK * 128 + k * 32), kk > 0 ? 1u : 0u);
         }
-        tc::mbar_init(kv_full, 1);
-        tc::fence_barrier_init();
-    }
-    if (warp == 0) {
-        tc::tmem_alloc(tmem_slot, 512);
-        tc::tmem_relinquish();
-    }
-    for (int i = threadIdx.x; i < 2 * 16 * 8; i += blockDim.x) {      // ones rows under V^T (outside the TMA boxes)
-        const int ch = i & 7, r = (i >> 3) & 15, sl = i >> 7;
-        *reinterpret_cast<uint4*>(sV + sl * V_SLAB + (NV + r) * 128 + ch * 16) =
-            make_uint4(0x3C003C00u, 0x3C003C00u, 0x3C003C00u, 0x3C003C00u);
-    }
-    fence_async_smem();
-    tc::fence_before_sync();
-    __syncthreads();
-    tc::fence_after_sync();
-    const uint32_t tmem_base = *tmem_slot;
-    rf_pdl_wait();         // prologue done; the producer grid must be complete before Q / K / V are read
-    const int n_mine = w1 - w0;
-
-    if (warp == 0 && lane == 0 && n_mine > 0) {
-        // ------------------------------------------------------------------ control thread: TMA + MMA issue
-        constexpr uint32_t idesc_qk = tc::make_idesc_f16(TQ, TK);
-        constexpr uint32_t idesc_pv = tc::make_idesc_f16(TQ, NVP);
-        const uint32_t k_lo = tc::desc_lo_sw128(tc::smem_u32(sK)), v_lo = tc::desc_lo_sw128(tc::smem_u32(sV));
-        auto load_q = [&](int n) {               // item w0+n -> Q buffer n&1
-            const int w = w0 + n, i = n & 1;
-            const int q_blk = w % nqb, head = (w / nqb) % p.heads, b = w / (nqb * p.heads);
-            if (n >= 2) tc::mbar_wait(&q_empty[i], ((n >> 1) - 1) & 1);   // Q K^T of item n-2 has completed
-            tc::mbar_expect_tx(&q_full[i], Q_BYTES);
+        tc::wgmma_commit();
+        tc::wgmma_wait<0>();
+        tc::reg_fence<TK / 2>(s);
+        // ---- mask keys beyond Nk (zero-filled by TMA) and, causal, beyond the query index
+        const int kmax0 = p.causal ? min(p.Nk, q0 + 1) : p.Nk, kmax1 = p.causal ? min(p.Nk, q1 + 1) : p.Nk;
+        float mt0 = -INFINITY, mt1 = -INFINITY;
 #pragma unroll
-            for (int s = 0; s < NSLAB; ++s)
-                tc::tma_load_4d(&mapQ, &q_full[i], sQ + i * Q_BYTES + s * TQ * 128, s * 64, q_blk * TQ, head, b);
-        };
-        auto issue_pv = [&](int n) {             // O_{n&1} = P_n V
-            const int i = n & 1;
-            tc::mbar_wait(&p_full[i], (n >> 1) & 1);
-            tc::fence_after_sync();
-            const uint32_t p_lo = tc::desc_lo_sw128(tc::smem_u32(sP + i * P_BYTES));
+        for (int i = 0; i < TK / 8; ++i) {
 #pragma unroll
-            for (int s = 0; s < 2; ++s)
-#pragma unroll
-                for (int k = 0; k < 4; ++k)
-                    tc::mma_f16_lo(tmem_base + 256 + i * NVP, p_lo + ((s * TQ * 128 + k * 32) >> 4),
-                                   v_lo + ((s * V_SLAB + k * 32) >> 4), idesc_pv, (s | k) ? 1u : 0u);
-            tc::mma_commit(&o_full[i]);
-        };
-        int cur_head = -1, kv_phase = 0;
-        load_q(0);
-        for (int n = 0; n < n_mine; ++n) {
-            const int w = w0 + n, i = n & 1;
-            const int head_id = w / nqb;         // (image, head) pair
-            if (n + 1 < n_mine) load_q(n + 1);
-            if (head_id != cur_head) {
-                // K / V^T are single buffered: everything issued for the previous head must have completed
-                if (n > 0) {
-                    issue_pv(n - 1);
-                    tc::mbar_wait(&o_full[(n - 1) & 1], ((n - 1) >> 1) & 1);
-                }
-                const int head = head_id % p.heads, b = head_id / p.heads;
-                tc::mbar_expect_tx(kv_full, K_BYTES + 2 * NV * 128);
-#pragma unroll
-                for (int s = 0; s < NSLAB; ++s) tc::tma_load_4d(&mapK, kv_full, sK + s * TK * 128, s * 64, 0, head, b);
-                tc::tma_load_4d(&mapVt, kv_full, sV, 0, 0, head, b);
-                tc::tma_load_4d(&mapVt, kv_full, sV + V_SLAB, 64, 0, head, b);
-                tc::mbar_wait(kv_full, kv_phase);
-                kv_phase ^= 1;
+            for (int e = 0; e < 2; ++e) {
+                const int key = j * TK + 8 * i + frag_col + e;
+                if (key >= kmax0) s[4 * i + e] = -INFINITY;
+                if (key >= kmax1) s[4 * i + 2 + e] = -INFINITY;
+                mt0 = fmaxf(mt0, s[4 * i + e]);
+                mt1 = fmaxf(mt1, s[4 * i + 2 + e]);
             }
-            // scores of item n (the softmax warps have pulled S of item n-2 into registers)
-            tc::mbar_wait(&q_full[i], (n >> 1) & 1);
-            if (n >= 2) tc::mbar_wait(&s_empty[i], ((n >> 1) - 1) & 1);
-            tc::fence_after_sync();
-            const uint32_t q_lo = tc::desc_lo_sw128(tc::smem_u32(sQ + i * Q_BYTES));
-#pragma unroll
-            for (int s = 0; s < NSLAB; ++s)
-#pragma unroll
-                for (int k = 0; k < 4; ++k)
-                    tc::mma_f16_lo(tmem_base + i * 128, q_lo + ((s * TQ * 128 + k * 32) >> 4),
-                                   k_lo + ((s * TK * 128 + k * 32) >> 4), idesc_qk, (s | k) ? 1u : 0u);
-            tc::mma_commit(&s_full[i]);
-            tc::mma_commit(&q_empty[i]);
-            // P V of the previous item, unless the head change above already issued it
-            if (n > 0 && head_id == cur_head) issue_pv(n - 1);
-            cur_head = head_id;
         }
-        issue_pv(n_mine - 1);
-    } else if (warp >= 1 && n_mine > 0) {
-        // ------------------------------------------------------------------ softmax + epilogue warps
-        const int q = (warp - 1) & 3;            // TMEM lane quarter == warp % 4 is NOT required here: see t_row
-        const int qq = warp & 3;                 // hardware: a warp may only touch TMEM lanes [32*(warp%4), +32)
-        const int row = qq * 32 + lane;
-        (void)q;
-        const uint32_t t_row = tmem_base + (static_cast<uint32_t>(qq * 32) << 16);
-        const float c = p.c;
-        auto epilogue = [&](int n) {
-            const int w = w0 + n, i = n & 1;
-            const int q_blk = w % nqb, head = (w / nqb) % p.heads, b = w / (nqb * p.heads);
-            tc::mbar_wait(&o_full[i], (n >> 1) & 1);
-            tc::fence_after_sync();
-            uint32_t l16[16];
-            tmem_ld16(t_row + 256 + i * NVP + NV, l16);
-            tc::tmem_wait_ld();
-            const float inv = 1.f / __uint_as_float(l16[0]);
-            const int qi = q_blk * TQ + row;
-            __half* dst = p.out + (static_cast<long>(b) * p.Nq + qi) * p.out_pitch + head * p.d;
-#pragma unroll 1
-            for (int c0 = 0; c0 < NV; c0 += 16) {
-                uint32_t o[16];
-                tmem_ld16(t_row + 256 + i * NVP + c0, o);
-                tc::tmem_wait_ld();
-                if (qi < p.Nq) {
+        mt0 = fmaxf(mt0, __shfl_xor_sync(0xffffffffu, mt0, 1));
+        mt0 = fmaxf(mt0, __shfl_xor_sync(0xffffffffu, mt0, 2));
+        mt1 = fmaxf(mt1, __shfl_xor_sync(0xffffffffu, mt1, 1));
+        mt1 = fmaxf(mt1, __shfl_xor_sync(0xffffffffu, mt1, 2));
+        const float mn0 = fmaxf(m0, mt0), mn1 = fmaxf(m1, mt1);
+        // a row that has seen no visible key yet keeps maximum -inf: use 0 as its reference so that exp2 gives 0, not NaN
+        const float r0 = mn0 == -INFINITY ? 0.f : mn0, r1 = mn1 == -INFINITY ? 0.f : mn1;
+        const float f0 = ex2((m0 - r0) * c), f1 = ex2((m1 - r1) * c);   // 0 on the first tile (m = -inf)
+        m0 = mn0;
+        m1 = mn1;
+        l0 *= f0;
+        l1 *= f1;
 #pragma unroll
-                    for (int ch = 0; ch < 2; ++ch) {
-                        const int col = c0 + 8 * ch;
-                        if (col < p.d) {
-                            uint32_t pk[4];
-#pragma unroll
-                            for (int e = 0; e < 4; ++e) {
-                                const __half2 h = __floats2half2_rn(__uint_as_float(o[8 * ch + 2 * e]) * inv,
-                                                                    __uint_as_float(o[8 * ch + 2 * e + 1]) * inv);
-                                pk[e] = *reinterpret_cast<const uint32_t*>(&h);
-                            }
-                            *reinterpret_cast<uint4*>(dst + col) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-                        }
-                    }
-                }
-            }
-            tc::fence_before_sync();
-        };
-        for (int n = 0; n < n_mine; ++n) {
-            const int i = n & 1;
-            tc::mbar_wait(&s_full[i], (n >> 1) & 1);
-            tc::fence_after_sync();
-            uint32_t v[128];
-#pragma unroll
-            for (int c0 = 0; c0 < 128; c0 += 32) {
-                if (c0 < ncols) {
-                    tc::tmem_ld_32x32(t_row + i * 128 + c0, v + c0);
-                } else {
-#pragma unroll
-                    for (int e = 0; e < 32; ++e) v[c0 + e] = 0xff800000u;
-                }
-            }
-            tc::tmem_wait_ld();
-            tc::fence_before_sync();
-            tc::mbar_arrive(&s_empty[i]);
-            const int kmax = p.causal ? min(p.Nk, ((w0 + n) % nqb) * TQ + row + 1) : p.Nk;   // causal: keys 0 .. query index
-#pragma unroll
-            for (int e = 0; e < 128; ++e)
-                if (e >= kmax) v[e] = 0xff800000u;
-            float mx[8];
-#pragma unroll
-            for (int e = 0; e < 8; ++e) mx[e] = __uint_as_float(v[e]);
-#pragma unroll
-            for (int e0 = 8; e0 < 128; e0 += 8)
-#pragma unroll
-                for (int e = 0; e < 8; ++e) mx[e] = fmaxf(mx[e], __uint_as_float(v[e0 + e]));
-            const float mt = fmaxf(fmaxf(fmaxf(mx[0], mx[1]), fmaxf(mx[2], mx[3])), fmaxf(fmaxf(mx[4], mx[5]), fmaxf(mx[6], mx[7])));
-            const float mc = mt * c;
-            uint8_t* myP = sP + i * P_BYTES;     // P buffer i was last read by P V of item n-2: its epilogue ran already
-#pragma unroll
-            for (int c0 = 0; c0 < 128; c0 += 8) {
-                uint32_t pk[4];
-                if (c0 < ncols) {
-#pragma unroll
-                    for (int e = 0; e < 8; e += 2) {
-                        float e0, e1;
-                        const float a0 = fmaf(__uint_as_float(v[c0 + e]), c, -mc);
-                        const float a1 = fmaf(__uint_as_float(v[c0 + e + 1]), c, -mc);
-                        asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e0) : "f"(a0));
-                        asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e1) : "f"(a1));
-                        const __half2 h = __floats2half2_rn(e0, e1);
-                        pk[e >> 1] = *reinterpret_cast<const uint32_t*>(&h);
-                    }
-                } else {
-                    pk[0] = pk[1] = pk[2] = pk[3] = 0u;
-                }
-                const int slab = c0 >> 6, chunk = (c0 & 63) >> 3;
-                *reinterpret_cast<uint4*>(myP + slab * TQ * 128 + row * 128 + ((chunk ^ (row & 7)) << 4)) =
-                    make_uint4(pk[0], pk[1], pk[2], pk[3]);
-            }
-            fence_async_smem();
-            tc::fence_before_sync();
-            tc::mbar_arrive(&p_full[i]);
-            if (n > 0) epilogue(n - 1);
+        for (int i = 0; i < NV / 8; ++i) {
+            o[4 * i] *= f0;
+            o[4 * i + 1] *= f0;
+            o[4 * i + 2] *= f1;
+            o[4 * i + 3] *= f1;
         }
-        epilogue(n_mine - 1);
+        // ---- P = exp2(S c - m c) in fp16, packed as the register A fragments of the P V product
+        const float mc0 = r0 * c, mc1 = r1 * c;
+        uint32_t pa[TK / 4];
+#pragma unroll
+        for (int i = 0; i < TK / 8; ++i) {
+            const uint32_t h0 = pack_half2(ex2(fmaf(s[4 * i], c, -mc0)), ex2(fmaf(s[4 * i + 1], c, -mc0)));
+            const uint32_t h1 = pack_half2(ex2(fmaf(s[4 * i + 2], c, -mc1)), ex2(fmaf(s[4 * i + 3], c, -mc1)));
+            const float2 g0 = __half22float2(*reinterpret_cast<const __half2*>(&h0));
+            const float2 g1 = __half22float2(*reinterpret_cast<const __half2*>(&h1));
+            l0 += g0.x + g0.y;
+            l1 += g1.x + g1.y;
+            pa[2 * i] = h0;
+            pa[2 * i + 1] = h1;
+        }
+        // ---- O += P V_j
+        const uint32_t v_base = tc::smem_u32(sV + st * V_BYTES);
+        tc::wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < TK / 16; ++kk)
+            tc::wgmma_rs<NV>(o, pa + 4 * kk, tc::make_desc_sw128(v_base + kk * 32), 1u);
+        tc::wgmma_commit();
+        tc::wgmma_wait<0>();
+        tc::reg_fence<NV / 2>(o);
+        tc::mbar_arrive(&kv_empty[st]);
     }
-    __syncthreads();
-    if (warp == 0) {
-        tc::fence_after_sync();
-        tc::tmem_dealloc(tmem_base, 512);
+    // ---- epilogue: O / rowsum -> fp16
+    l0 += __shfl_xor_sync(0xffffffffu, l0, 1);
+    l0 += __shfl_xor_sync(0xffffffffu, l0, 2);
+    l1 += __shfl_xor_sync(0xffffffffu, l1, 1);
+    l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
+    const float inv0 = 1.f / l0, inv1 = 1.f / l1;
+    __half* dst0 = p.out + (static_cast<long>(b) * p.Nq + q0) * p.out_pitch + head * p.d;
+    __half* dst1 = dst0 + 8 * p.out_pitch;
+#pragma unroll
+    for (int i = 0; i < NV / 8; ++i) {
+        const int col = 8 * i + frag_col;
+        if (col < p.d) {
+            if (q0 < p.Nq) *reinterpret_cast<uint32_t*>(dst0 + col) = pack_half2(o[4 * i] * inv0, o[4 * i + 1] * inv0);
+            if (q1 < p.Nq) *reinterpret_cast<uint32_t*>(dst1 + col) = pack_half2(o[4 * i + 2] * inv1, o[4 * i + 3] * inv1);
+        }
     }
 }
 
@@ -999,55 +244,15 @@ template <int DPAD, int NV, int NS>
 int launch_attn(const CUtensorMap& mq, const CUtensorMap& mk, const CUtensorMap& mv, const AttnParams& p, dim3 grid,
                 cudaStream_t st) {
     constexpr int NSLAB = DPAD / 64;
-    constexpr int V_SLAB = ((NV * 128 + 1023) / 1024) * 1024;
-    const size_t smem = static_cast<size_t>(NSLAB) * TQ * 128 + static_cast<size_t>(NS) * (NSLAB * TK * 128 + 2 * V_SLAB) +
-                        2 * (2 * TQ * 128) + 256 + 2 * 128 * 4 + 1024;
+    constexpr int V_BYTES = ((NV * 128 + 1023) / 1024) * 1024;
+    constexpr size_t smem = static_cast<size_t>(NSLAB) * TQ * 128 + static_cast<size_t>(NS) * (NSLAB * TK * 128 + V_BYTES) +
+                            256 + 1024;
+    static_assert(smem <= 232448, "shared memory budget (227 KB per block)");
     static rf_dev_once once;
     const cudaError_t aerr = rf_set_smem_once(once, k_flash_attn<DPAD, NV, NS>, int(smem));
     if (aerr != cudaSuccess) return rf_fail(RF_ERR_CUDA, std::string("cudaFuncSetAttribute(k_flash_attn): ") + cudaGetErrorString(aerr));
-    RF_LAUNCH_PDL("k_flash_attn", (k_flash_attn<DPAD, NV, NS>), grid, dim3(320), smem, st, grid.x * grid.y * grid.z <= 600u, mq, mk, mv, p);
-    return RF_OK;
-}
-
-template <int DPAD, int NV, int NKS, int NVS, int NG>
-int launch_attn1(const CUtensorMap& mq, const CUtensorMap& mk, const CUtensorMap& mv, const AttnParams& p, dim3 grid,
-                 cudaStream_t st) {
-    constexpr int NSLAB = DPAD / 64, TKT = 256 / NG, KSL = TKT / 64;
-    constexpr int V_SLAB = (((NV + 16) * 128 + 1023) / 1024) * 1024;
-    constexpr size_t smem = static_cast<size_t>(NSLAB) * TQ * 128 + static_cast<size_t>(NKS) * NSLAB * TKT * 128 +
-                            static_cast<size_t>(NVS) * KSL * V_SLAB + static_cast<size_t>(NG) * KSL * TQ * 128 + 512 +
-                            NG * 128 * 4 + 1024;
-    static_assert(smem <= 232448, "shared memory budget");
-    static rf_dev_once once;
-    const cudaError_t aerr = rf_set_smem_once(once, k_flash_attn1<DPAD, NV, NKS, NVS, NG>, int(smem));
-    if (aerr != cudaSuccess) return rf_fail(RF_ERR_CUDA, std::string("cudaFuncSetAttribute(k_flash_attn1): ") + cudaGetErrorString(aerr));
-    RF_LAUNCH_PDL("k_flash_attn1", (k_flash_attn1<DPAD, NV, NKS, NVS, NG>), grid, dim3(96 + 128 * NG), smem, st,
+    RF_LAUNCH_PDL("k_flash_attn", (k_flash_attn<DPAD, NV, NS>), grid, dim3(ATTN_THREADS), smem, st,
                   grid.x * grid.y * grid.z <= 600u, mq, mk, mv, p);
-    return RF_OK;
-}
-
-template <int DPAD, int NV>
-int launch_attn_short(const CUtensorMap& mq, const CUtensorMap& mk, const CUtensorMap& mv, const AttnParams& p, int B,
-                      cudaStream_t st) {
-    constexpr int NSLAB = DPAD / 64;
-    constexpr int V_SLAB = (((NV + 16) * 128 + 1023) / 1024) * 1024;
-    constexpr size_t smem = 2 * static_cast<size_t>(NSLAB) * TQ * 128 + static_cast<size_t>(NSLAB) * TK * 128 + 2 * V_SLAB +
-                            2 * (2 * TQ * 128) + 256 + 1024;
-    static_assert(smem <= 232448, "shared memory budget");
-    static rf_dev_once once;
-    const cudaError_t aerr = rf_set_smem_once(once, k_attn_short<DPAD, NV>, int(smem));
-    static int num_sms = 0;
-    if (!num_sms) {
-        int dev = 0, n = 148;
-        if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-        num_sms = n;
-    }
-    if (aerr != cudaSuccess) return rf_fail(RF_ERR_CUDA, std::string("cudaFuncSetAttribute(k_attn_short): ") + cudaGetErrorString(aerr));
-    const int nqb = (p.Nq + TQ - 1) / TQ;
-    const int n_items = nqb * p.heads * B;
-    const int grid = n_items < num_sms ? n_items : num_sms;
-    RF_LAUNCH_PDL("k_attn_short", (k_attn_short<DPAD, NV>), dim3(grid), dim3(160), smem, st, n_items <= 4 * num_sms, mq, mk, mv, p,
-                  n_items, nqb);
     return RF_OK;
 }
 
@@ -1061,7 +266,7 @@ extern "C" int rf_attention_f16(const void* q, const void* k, const void* vt, vo
 
 extern "C" int rf_attention_masked_f16(const void* q, const void* k, const void* vt, void* out, int B, int heads, int Nq,
                                        int Nk, int d, int vt_pitch, float scale, int causal, void* stream) {
-    if (causal && (Nk > TK || d > 112))
+    if (causal && (Nk > 128 || d > 112))
         return rf_fail(RF_ERR_UNSUPPORTED, "rf_attention_masked_f16: the causal mask is implemented for Nk <= 128, d <= 112 "
                                            "(the 77-token text encoder)");
     if (!q || !k || !vt || !out || B <= 0 || heads <= 0 || Nq <= 0 || Nk <= 0 || d <= 0 || (d % 8) || vt_pitch < Nk ||
@@ -1069,12 +274,6 @@ extern "C" int rf_attention_masked_f16(const void* q, const void* k, const void*
         return rf_fail(RF_ERR_INVALID, "rf_attention_f16: bad argument");
     if (d > 192) return rf_fail(RF_ERR_UNSUPPORTED, "rf_attention_f16: head dim > 192 (use the GEMM + softmax path)");
     const long C = static_cast<long>(heads) * d;
-    static const bool two_pass = getenv("RF_ATTN_TWO_PASS") != nullptr;   // A/B switch for the older kernel
-    static const bool two_groups = getenv("RF_ATTN_TWO_GROUPS") != nullptr;     // A/B switch (four groups: 766 vs 830 us)
-    const bool one_pass = !two_pass && d <= 112;
-    const bool short_keys = one_pass && Nk <= TK && getenv("RF_ATTN_NO_SHORT") == nullptr;
-    const int ng = (one_pass && d <= 48 && !two_groups && !short_keys) ? 4 : 2;   // softmax groups; key tile = 256 / ng keys
-    const int tkt = one_pass ? 256 / ng : TK;
     CUtensorMap mq, mk, mv;
     {
         const long dims[4] = {d, Nq, heads, B};
@@ -1086,7 +285,7 @@ extern "C" int rf_attention_masked_f16(const void* q, const void* k, const void*
     {
         const long dims[4] = {d, Nk, heads, B};
         const long str[4] = {1, C, d, static_cast<long>(Nk) * C};
-        const int box[4] = {64, tkt, 1, 1};
+        const int box[4] = {64, TK, 1, 1};
         int rc = map4(&mk, k, dims, str, box);
         if (rc) return rc;
     }
@@ -1095,49 +294,26 @@ extern "C" int rf_attention_masked_f16(const void* q, const void* k, const void*
     {
         const long dims[4] = {Nk, d, heads, B};
         const long str[4] = {1, vt_pitch, static_cast<long>(d) * vt_pitch, C * vt_pitch};
-        const int box[4] = {64, NV, 1, 1};
+        const int box[4] = {TK, NV, 1, 1};
         int rc = map4(&mv, vt, dims, str, box);
         if (rc) return rc;
     }
     AttnParams p;
     p.Nq = Nq; p.Nk = Nk; p.d = d; p.heads = heads;
-    p.n_tiles = (Nk + tkt - 1) / tkt;
+    p.n_tiles = (Nk + TK - 1) / TK;
     p.c = scale * 1.4426950408889634f;
     p.out = static_cast<__half*>(out);
     p.out_pitch = C;
     p.causal = causal ? 1 : 0;
-    {
-        // measured at the benchmarked batch (profiles/README.md, round 2): 73.8 ms per evaluation with the polynomial on,
-        // 71.3 ms off — the softmax warps are FMA/ALU-issue bound before they are MUFU bound, so moving exponentials to
-        // the FMA pipe loses.  Kept as an experiment switch (RF_ATTN_POLY=1), off by default.
-        const char* e = getenv("RF_ATTN_POLY");
-        p.poly_exp = (e && e[0] == '1') ? 1 : 0;
-    }
     dim3 grid((Nq + TQ - 1) / TQ, heads, B);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    static const bool no_short = getenv("RF_ATTN_NO_SHORT") != nullptr;
-    if (one_pass && Nk <= TK && (!no_short || causal)) {     // one key tile: persistent kernel (cross-attention to the text tokens)
-        if (d <= 48) return launch_attn_short<64, 48>(mq, mk, mv, p, B, st);
-        if (d <= 64) return launch_attn_short<64, 64>(mq, mk, mv, p, B, st);
-        if (d <= 80) return launch_attn_short<128, 80>(mq, mk, mv, p, B, st);
-        if (d <= 96) return launch_attn_short<128, 96>(mq, mk, mv, p, B, st);
-        return launch_attn_short<128, 112>(mq, mk, mv, p, B, st);
-    }
-    if (one_pass) {
-        // ring depths fill the 227 KB of shared memory next to Q and the P tiles
-        if (ng == 4) return launch_attn1<64, 48, 8, 6, 4>(mq, mk, mv, p, grid, st);
-        if (d <= 48) return launch_attn1<64, 48, 4, 3, 2>(mq, mk, mv, p, grid, st);
-        if (d <= 64) return launch_attn1<64, 64, 4, 3, 2>(mq, mk, mv, p, grid, st);
-        if (d <= 80) return launch_attn1<128, 80, 2, 2, 2>(mq, mk, mv, p, grid, st);
-        if (d <= 96) return launch_attn1<128, 96, 2, 2, 2>(mq, mk, mv, p, grid, st);
-        return launch_attn1<128, 112, 2, 2, 2>(mq, mk, mv, p, grid, st);
-    }
-    if (d <= 48) return launch_attn<64, 48, 3>(mq, mk, mv, p, grid, st);
-    if (d <= 64) return launch_attn<64, 64, 3>(mq, mk, mv, p, grid, st);
-    if (d <= 80) return launch_attn<128, 80, 2>(mq, mk, mv, p, grid, st);
-    if (d <= 96) return launch_attn<128, 96, 2>(mq, mk, mv, p, grid, st);
-    if (d <= 112) return launch_attn<128, 112, 2>(mq, mk, mv, p, grid, st);
-    if (d <= 128) return launch_attn<128, 128, 2>(mq, mk, mv, p, grid, st);
-    if (d <= 160) return launch_attn<192, 160, 1>(mq, mk, mv, p, grid, st);
-    return launch_attn<192, 192, 1>(mq, mk, mv, p, grid, st);
+    // ring depths: as many K / V^T stages as keep two CTAs' worth of shared memory per SM for the small head dims
+    if (d <= 48) return launch_attn<64, 48, 4>(mq, mk, mv, p, grid, st);
+    if (d <= 64) return launch_attn<64, 64, 4>(mq, mk, mv, p, grid, st);
+    if (d <= 80) return launch_attn<128, 80, 3>(mq, mk, mv, p, grid, st);
+    if (d <= 96) return launch_attn<128, 96, 3>(mq, mk, mv, p, grid, st);
+    if (d <= 112) return launch_attn<128, 112, 3>(mq, mk, mv, p, grid, st);
+    if (d <= 128) return launch_attn<128, 128, 3>(mq, mk, mv, p, grid, st);
+    if (d <= 160) return launch_attn<192, 160, 2>(mq, mk, mv, p, grid, st);
+    return launch_attn<192, 192, 2>(mq, mk, mv, p, grid, st);
 }

@@ -1,5 +1,5 @@
 // Path (a) kernels + C-ABI: STFT / iSTFT / Griffin-Lim / mel / inverse mel / quantisation.
-// sm_100a only.  See DESIGN.md §3 for the algorithm and data layout.
+// sm_90a only.  See DESIGN.md §3 for the algorithm and data layout.
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -25,7 +25,7 @@ int rf_fail(int code, const std::string& msg) {
     return code;
 }
 extern "C" const char* rf_last_error(void) { return g_rf_err.c_str(); }
-extern "C" const char* rf_version(void) { return "rf_b200 0.1 (sm_100a)"; }
+extern "C" const char* rf_version(void) { return "rf_b200 0.1 (sm_90a)"; }
 
 // ---------------------------------------------------------------------------------------
 // plan object
@@ -105,8 +105,8 @@ static int rf_plan_upload(rf_plan* p) {
     RF_CUDA_TRY(cudaGetDevice(&dev));
     cudaDeviceProp prop;
     RF_CUDA_TRY(cudaGetDeviceProperties(&prop, dev));
-    if (prop.major != 10)
-        return rf_fail(RF_ERR_CUDA, std::string("rf_b200: kernels are built for sm_100a only; device is ") +
+    if (prop.major != 9 || prop.minor != 0)
+        return rf_fail(RF_ERR_CUDA, std::string("rf_b200: kernels are built for sm_90a only; device is ") +
                                         prop.name);
     const rf_plan_host& h = p->h;
     RF_CUDA_TRY(upload_tabs(p, &p->d10, h.t10));

@@ -48,16 +48,14 @@ inline cudaError_t rf_set_smem_once(rf_dev_once& o, F* func, int bytes) {
 // ---------------------------------------------------------------------------------------------------------------------
 // Programmatic dependent launch (PDL).  A CFG UNet evaluation is ~440 dependent launches; with the attribute below the
 // next kernel's CTAs are scheduled as soon as every CTA of the current one has passed rf_pdl_trigger(), run their prologue
-// (barrier init, TMEM allocation, descriptor prefetch) and then block in rf_pdl_wait() until the current grid has
-// completed and its writes are visible.  Rules that keep this safe:
+// (barrier init, descriptor prefetch) and then block in rf_pdl_wait() until the current grid has completed and its
+// writes are visible.  Rules that keep this safe:
 //   * a kernel launched through RF_LAUNCH_PDL executes rf_pdl_wait() in EVERY thread before its first global-memory access
 //     (reads of the producer's output and writes that could overtake the producer's reads alike);
 //   * everything else is launched the ordinary way and therefore still waits for full completion of its predecessor.
-// Measured on the B200 (scratch/r2_run16.sh, one CFG evaluation as a CUDA graph, attribute on every launch): 2 images
-// 5.80 -> 5.55 ms (-4 %), 64 images 72.7 -> 73.7 ms (+1 %: at the benchmarked batch the kernels are long, and early-resident
-// dependents only take resources from the tail of the running grid).  Hence the default mode: the attribute goes on launches
-// that cannot fill the GPU anyway (`small`: a couple of waves at most — the single-request regime) and stays off otherwise
-// (second run, same script: 64 images 68.60 / 68.36 / 69.22 ms and 2 images 5.89 / 5.60 / 5.59 ms for RF_PDL = 0 / 1 / 2).
+// Early-resident dependents hide launch latency when the kernels are short, but at large batches they only take
+// resources from the tail of the running grid.  Hence the default mode: the attribute goes on launches that cannot fill
+// the GPU anyway (`small`: a couple of waves at most — the single-request regime) and stays off otherwise.
 // RF_PDL in the environment: 0 = never, 1 = small launches (default), 2 = every instrumented launch.  Without the attribute
 // the device instructions are no-ops.
 #include <cstdlib>

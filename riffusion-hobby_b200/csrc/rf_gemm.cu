@@ -1,11 +1,11 @@
-// Path (b) tensor-core workhorse: one tcgen05/TMEM kernel that computes
+// Path (b) tensor-core workhorse: one wgmma / TMA kernel that computes
 //     D[b][m][n] = act(alpha * sum_k A[b][m][k] * B[b][n][k] + bias) + residual          (fp16 in, fp32 accumulate)
 // either as a batched "TN" GEMM (both operands K-major; linears, 1x1 convs, QK^T, PV) or as an
 // implicit-GEMM 3x3 / strided convolution over NHWC activations (the im2col gather is done by the
 // TMA engine: one 4-D box load per filter tap with out-of-bounds zero fill supplying the padding).
 //
-// CTA = one 128 x BN output tile.  Warp roles: warp 0 = TMA producer (one thread), warp 1 = TMEM
-// allocation + MMA issue (one thread), warps 2-5 = epilogue (TMEM -> registers -> global).
+// CTA = one 128 x BN output tile at a time.  Warp roles: warps 0-7 = two consumer warpgroups (rows 0-63 / 64-127 of the
+// tile: wgmma m64nBNk16 with both operands in shared memory, then the epilogue), warp 8 = TMA producer (one thread).
 // K is streamed in 64-element (128-byte, SWIZZLE_128B) slabs through a STAGES-deep mbarrier ring.
 //
 // Reference arithmetic this replaces (diffusers 0.9 modules reached from
@@ -15,6 +15,7 @@
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <cstdio>
 #include <cstdlib>
 #include <mutex>
@@ -29,11 +30,10 @@ namespace {
 constexpr int BM = 128;
 constexpr int BK = 64;
 constexpr int A_TILE_BYTES = BM * BK * 2;  // 16 KB
-// epilogue warp sets (4 warps = the 4 TMEM lane quarters each); set s drains the 32-column runs s, s + EPI_SETS, ...
-// Four sets: a 128-column tile is drained in one run per warp — the K <= 640 GEMMs are epilogue bound (MMA 0.8 us vs
-// ~4 us of tcgen05.ld / convert / store per tile with two sets).
-constexpr int EPI_SETS = 4;
-constexpr int GEMM_THREADS = 64 + 128 * EPI_SETS;
+constexpr int GEMM_THREADS = 256 + 32;     // two consumer warpgroups + one producer warp
+constexpr int STAGE_PAD = 4;               // fp32 staging row pitch BN + 4: row-per-thread float4 reads are conflict free
+
+__host__ __device__ constexpr int stage_bytes(int BN) { return BM * (BN + STAGE_PAD) * 4; }
 
 struct TcParams {
     // problem
@@ -84,8 +84,7 @@ __device__ __forceinline__ float apply_act(float v, int act) {
 //   0.5 erfc(t) = 2^q(t) on t = |g| / sqrt 2 in [0, 4] (degree-7 fit of -log2 erfc(t) - 1; erfc(4) = 1.5e-8, clamped
 //   beyond), Phi = g < 0 ? h : 1 - h.  |error| <= 7e-7 absolute, <= 4.2e-6 relative (fp32 Horner), i.e. 1 % of an fp16 ulp —
 //   same function as erff's GELU (diffusers GEGLU uses the exact form), not the tanh approximation.  erff() costs ~35
-//   instructions per element on two divergent paths and made the K = 320 GEGLU GEMM epilogue-bound (ALU ~4500 clk per
-//   tile against 2560 clk of MMA).
+//   instructions per element on two divergent paths.
 __device__ __forceinline__ float gelu_erf_fast(float g) {
     const float t = fminf(fabsf(g) * 0.70710678118654752f, 4.0f);
     float q = -2.1777638e-05f;
@@ -101,99 +100,61 @@ __device__ __forceinline__ float gelu_erf_fast(float g) {
     return g * (g < 0.f ? h : 1.f - h);
 }
 
-// Persistent kernel: grid = min(#tiles, #SMs) CTAs, each walking tiles t = blockIdx.x, +gridDim.x, ...
-//   warp 0: TMA producer — streams the K slabs of all its tiles through one STAGES-deep ring (phases run across tiles)
-//   warp 1: MMA issuer  — accumulates tile i in TMEM buffer i&1, commits tmem_full[i&1]
-//   warps 2-17: epilogue (4 sets x 4 warps) — drain buffer i&1 (tcgen05.ld -> bias/act/residual -> global) while the MMA warp already works
-//              on tile i+1 in the other buffer; arrive tmem_empty[i&1] (256 threads) when done
+__device__ __forceinline__ void named_bar_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
+
+// Persistent kernel: grid = min(#tiles, #SMs) CTAs, each walking work units t = blockIdx.x, +gridDim.x, ...
+//   warp 8:    TMA producer — streams the K slabs of all its units through one STAGES-deep ring (phases run across units)
+//   warps 0-7: two consumer warpgroups — wgmma into register accumulators, releasing each ring stage as soon as the MMAs
+//              that read it have completed; then the accumulators go through an fp32 staging tile in shared memory to a
+//              row-per-thread epilogue (bias / activation / residual / GEGLU / split-K partials).  The producer keeps
+//              filling the ring for the next unit while the epilogue runs.
 // Tile order: n fastest, then m, then batch, so CTAs running at the same time share activation rows in L2.
 //
-// PAIR = true: the same kernel for a CTA pair (cluster of 2, cta_group::2).  A work unit is a 256 x BN tile: CTA rank r owns
-// the 128-row block m_blk = 2 * pair_row + r (its own A rows, its own TMEM accumulator rows, its own epilogue) and stages
-// only columns [r * BN/2, +BN/2) of the B tile; the leader (rank 0) issues one 256-row MMA per K step that reads both CTAs'
-// shared memory.  Barriers: the TMA loads of both CTAs credit the leader's full[stage]; the leader's MMA commits are
-// multicast to empty[stage] / tmem_full[acc] of both CTAs; both epilogues arrive on the leader's tmem_empty[acc].
-//
-// SLABS = 64-element K slabs per ring stage.  scratch/mma_bench.cu (profiles/r02_mma_issue_rate.txt): with the operands
-// resident and NO data movement, one full-barrier wait + tcgen05 fence + commit per 4 MMAs already costs ~135 cycles of
-// tensor-pipe idle time per round trip (N = 160: 457 cycles per slab against 320 ideal = 70 %; 8 MMAs per round trip:
-// 82 %; 12: 99 %), so a stage carries two (or three) slabs and the issuer commits once per stage.
-//
-// BRES = true (1-SM, K <= BRES_KB slabs, non-batched): B-stationary.  A CTA stays on ONE column block, loads all K slabs of
-// its B tile into shared memory once and streams only A through the ring while it walks the row blocks.  For the K = N = 320
-// projections of the 64x64 level (35 launches per evaluation) the weight tile (100 KB) was re-fetched from L2 for every
-// 128-row block: 180 KB of operands per 1600 cycles of MMA, L2-feed bound at 440-450 TFLOP/s; resident B leaves 80 KB.
+// BRES = true (K <= BRES_KB slabs, non-batched): B-stationary.  A CTA stays on ONE column block, loads all K slabs of its
+// B tile into shared memory once and streams only A through the ring while it walks the row blocks: the weight tile is
+// not re-fetched from L2 for every 128-row block of the K <= 320 projections.
 constexpr int BRES_KB = 5;
-template <int BN, int STAGES, bool PAIR, int SLABS, bool BRES = false>
+template <int BN, int STAGES, bool BRES = false>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 k_tc_gemm(const __grid_constant__ CUtensorMap mapA0, const __grid_constant__ CUtensorMap mapA1,
           const __grid_constant__ CUtensorMap mapB, const TcParams p) {
     extern __shared__ __align__(1024) uint8_t smem[];
     rf_pdl_trigger();      // the next kernel may start its prologue; it blocks in its own rf_pdl_wait() until this grid is done
-    // BN = 320 (pairs only): two 160-wide MMA instructions per K step share the A operand; the 320 accumulator columns
-    // leave no room for a second set, so the epilogue of a tile does not overlap the next tile's MMAs (NBUF = 1) —
-    // worth it for long K: 56 B/clk of operands per SM instead of 115 (the 1-SM 128 x 160 tile is L2-feed bound).
-    static_assert(BN != 320 || PAIR, "320-wide tiles exist for CTA pairs only");
-    constexpr int UN = BN == 320 ? 160 : BN;        // MMA instruction width
-    constexpr int NI = BN / UN;                     // instructions per K step
-    constexpr int NBUF = BN == 320 ? 1 : 2;         // TMEM accumulator sets
-    constexpr int B_TILE_BYTES = (PAIR ? BN / 2 : BN) * BK * 2;
-    constexpr int ACC_COLS = BN <= 32 ? 32 : BN <= 64 ? 64 : BN <= 128 ? 128 : BN <= 256 ? 256 : 512;   // powers of two
-    static_assert(!BRES || !PAIR, "B-stationary mode is a 1-SM mode");
-    uint8_t* sA = smem;                                      // [STAGES][SLABS][A_TILE_BYTES]
-    uint8_t* sB = smem + STAGES * SLABS * A_TILE_BYTES;      // [STAGES][SLABS][B_TILE_BYTES], BRES: [BRES_KB][B_TILE_BYTES] resident
-    uint64_t* full = reinterpret_cast<uint64_t*>(smem + STAGES * SLABS * A_TILE_BYTES +
-                                                 (BRES ? BRES_KB : STAGES * SLABS) * B_TILE_BYTES);
+    constexpr int B_TILE_BYTES = BN * BK * 2;
+    constexpr int PITCH = BN + STAGE_PAD;
+    uint8_t* sA = smem;                                      // [STAGES][A_TILE_BYTES]
+    uint8_t* sB = smem + STAGES * A_TILE_BYTES;              // [STAGES][B_TILE_BYTES], BRES: [BRES_KB][B_TILE_BYTES] resident
+    float* stg = reinterpret_cast<float*>(sB + (BRES ? BRES_KB : STAGES) * B_TILE_BYTES);   // [BM][PITCH]
+    uint64_t* full = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(stg) + stage_bytes(BN));
     uint64_t* empty = full + STAGES;
-    uint64_t* tmem_full = empty + STAGES;      // [2]
-    uint64_t* tmem_empty = tmem_full + 2;      // [2]
-    uint64_t* b_full = tmem_empty + 2;         // BRES: the resident B tile has landed
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(b_full + 1);
+    uint64_t* b_full = empty + STAGES;          // BRES: the resident B tile has landed
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    // PAIR: tiles_m counts 256-row blocks (the host passes ceil(tiles_m / 2)); work units are walked by the pair
     const int tiles_mn = p.tiles_n * p.tiles_m;
     const int n_tiles = tiles_mn * p.batch1 * p.batch2 * p.splits;   // work units (== tiles when splits == 1)
-    const int rank = PAIR ? static_cast<int>(tc::cluster_ctarank()) : 0;
     // BRES: the CTA owns column block nb_fixed and walks row blocks unit = blockIdx.x / tiles_n, + gridDim.x / tiles_n, ...
     const int nb_fixed = BRES ? static_cast<int>(blockIdx.x) % p.tiles_n : 0;
-    const int unit0 = BRES ? static_cast<int>(blockIdx.x) / p.tiles_n : (PAIR ? blockIdx.x >> 1 : blockIdx.x);
-    const int unit_step = BRES ? static_cast<int>(gridDim.x) / p.tiles_n : (PAIR ? gridDim.x >> 1 : gridDim.x);
+    const int unit0 = BRES ? static_cast<int>(blockIdx.x) / p.tiles_n : blockIdx.x;
+    const int unit_step = BRES ? static_cast<int>(gridDim.x) / p.tiles_n : gridDim.x;
     const int n_units = BRES ? p.tiles_m : n_tiles;
 
     if (threadIdx.x == 0) {
         for (int i = 0; i < STAGES; ++i) {
             tc::mbar_init(&full[i], 1);
-            tc::mbar_init(&empty[i], 1);
-        }
-        for (int i = 0; i < 2; ++i) {
-            tc::mbar_init(&tmem_full[i], 1);
-            tc::mbar_init(&tmem_empty[i], (PAIR ? 2 : 1) * 4 * EPI_SETS);   // one arrival per epilogue warp (of both CTAs)
+            tc::mbar_init(&empty[i], 256);      // every consumer thread arrives once it is done with the stage
         }
         tc::mbar_init(b_full, 1);
         tc::fence_barrier_init();
     }
-    if (warp == 0 && lane == 0) {
+    if (warp == 8 && lane == 0) {
         tc::tma_prefetch_desc(&mapA0);
         tc::tma_prefetch_desc(&mapB);
     }
-    if (warp == 1) {
-        if constexpr (PAIR) {
-            tc::tmem_alloc_pair(tmem_slot, NBUF * ACC_COLS);
-            tc::tmem_relinquish_pair();
-        } else {
-            tc::tmem_alloc(tmem_slot, NBUF * ACC_COLS);
-            tc::tmem_relinquish();
-        }
-    }
-    tc::fence_before_sync();
-    if constexpr (PAIR) tc::cluster_sync_all();   // the peer's barriers must be initialised before anything signals them
-    else __syncthreads();
-    tc::fence_after_sync();
-    const uint32_t tmem_base = *tmem_slot;
-    rf_pdl_wait();         // barriers, TMEM and descriptors are set up: from here on global memory is touched
+    __syncthreads();
+    rf_pdl_wait();         // barriers and descriptors are set up: from here on global memory is touched
 
-    if (warp == 0 && lane == 0) {
+    if (warp == 8) {
+        if (lane != 0) return;
         // ------------------------------------------------------------ TMA producer
         int it = 0;
         if constexpr (BRES) {      // the whole K extent of this CTA's B tile, once
@@ -205,8 +166,7 @@ k_tc_gemm(const __grid_constant__ CUtensorMap mapA0, const __grid_constant__ CUt
             const int tile = BRES ? unit * p.tiles_n + nb_fixed : unit / p.splits, sp = BRES ? 0 : unit - (unit / p.splits) * p.splits;
             const int kb0 = sp * p.kb_per_split, kb1 = min(p.num_kb, kb0 + p.kb_per_split);
             const int z = tile / tiles_mn, mn = tile - z * tiles_mn;
-            const int m_row = mn / p.tiles_n, n_blk = mn - m_row * p.tiles_n;
-            const int m_blk = PAIR ? 2 * m_row + rank : m_row;
+            const int m_blk = mn / p.tiles_n, n_blk = mn - m_blk * p.tiles_n;
             const int b1 = z % p.batch1, b2 = z / p.batch1;
             int tx = 0, ty = 0, tb = 0;
             if (p.conv) {
@@ -214,309 +174,235 @@ k_tc_gemm(const __grid_constant__ CUtensorMap mapA0, const __grid_constant__ CUt
                 ty = (m_blk / p.tiles_x) % p.tiles_y;
                 tb = m_blk / (p.tiles_x * p.tiles_y);
             }
-            const int n0 = n_blk * BN + ((PAIR && NI == 1) ? rank * (BN / 2) : 0);      // this CTA's rows of the B tile
-            for (int kbs = kb0; kbs < kb1; kbs += SLABS, ++it) {
+            for (int kb = kb0; kb < kb1; ++kb, ++it) {
                 const int stage = it % STAGES;
                 const uint32_t phase = (it / STAGES) & 1;
-                const int nsl = min(SLABS, kb1 - kbs);          // slabs of this stage (the last stage of a tile may be short)
                 tc::mbar_wait(&empty[stage], phase ^ 1);
-                // only the leader posts the byte count: the loads of BOTH CTAs are credited to its barrier
-                if (rank == 0)
-                    tc::mbar_expect_tx(&full[stage], (PAIR ? 2 : 1) * nsl * (A_TILE_BYTES + (BRES ? 0 : B_TILE_BYTES)));
-                const uint32_t fb = PAIR ? tc::mapa_u32(tc::smem_u32(&full[stage]), 0) : 0;
-              for (int sl = 0; sl < nsl; ++sl) {
-                const int kb = kbs + sl;
-                void* dstA = sA + (stage * SLABS + sl) * A_TILE_BYTES;
-                void* dstB = sB + (stage * SLABS + sl) * B_TILE_BYTES;
-                if constexpr (PAIR) {
-                    if (!p.conv) {
-                        tc::tma_load_4d_pair(&mapA0, fb, dstA, kb * BK, m_blk * BM, b1 * p.a_m1, b2 * p.a_m2);
-#pragma unroll
-                        for (int i = 0; i < NI; ++i)    // instruction i reads rows [i * UN/2, +UN/2) of this CTA's B stage
-                            tc::tma_load_4d_pair(&mapB, fb, static_cast<uint8_t*>(dstB) + i * (UN / 2) * BK * 2, kb * BK,
-                                                 n_blk * BN + i * UN + rank * (UN / 2), b1 * p.b_m1, b2 * p.b_m2);
-                    } else {
-                        const int kct = p.kc1 + p.kc2;
-                        const int tap = kb / kct, kc = kb - tap * kct;
-                        const int dy = tap / p.tap_w, dx = tap - dy * p.tap_w;
-                        const int x0 = tx * p.bw * p.stride + dx - p.pad + p.off_x;
-                        const int y0 = ty * p.bh * p.stride + dy - p.pad + p.off_y;
-                        if (kc < p.kc1)
-                            tc::tma_load_4d_pair(&mapA0, fb, dstA, kc * BK, x0, y0, tb * p.bb);
-                        else
-                            tc::tma_load_4d_pair(&mapA1, fb, dstA, (kc - p.kc1) * BK, x0, y0, tb * p.bb);
-#pragma unroll
-                        for (int i = 0; i < NI; ++i)
-                            tc::tma_load_4d_pair(&mapB, fb, static_cast<uint8_t*>(dstB) + i * (UN / 2) * BK * 2, kb * BK,
-                                                 n_blk * BN + i * UN + rank * (UN / 2), 0, 0);
-                    }
+                tc::mbar_expect_tx(&full[stage], A_TILE_BYTES + (BRES ? 0 : B_TILE_BYTES));
+                void* dstA = sA + stage * A_TILE_BYTES;
+                void* dstB = sB + stage * B_TILE_BYTES;
+                if (!p.conv) {
+                    tc::tma_load_4d(&mapA0, &full[stage], dstA, kb * BK, m_blk * BM, b1 * p.a_m1, b2 * p.a_m2);
+                    if (!BRES) tc::tma_load_4d(&mapB, &full[stage], dstB, kb * BK, n_blk * BN, b1 * p.b_m1, b2 * p.b_m2);
                 } else {
-                    if (!p.conv) {
-                        tc::tma_load_4d(&mapA0, &full[stage], dstA, kb * BK, m_blk * BM, b1 * p.a_m1, b2 * p.a_m2);
-                        if (!BRES) tc::tma_load_4d(&mapB, &full[stage], dstB, kb * BK, n0, b1 * p.b_m1, b2 * p.b_m2);
-                    } else {
-                        const int kct = p.kc1 + p.kc2;
-                        const int tap = kb / kct, kc = kb - tap * kct;
-                        const int dy = tap / p.tap_w, dx = tap - dy * p.tap_w;
-                        const int x0 = tx * p.bw * p.stride + dx - p.pad + p.off_x;
-                        const int y0 = ty * p.bh * p.stride + dy - p.pad + p.off_y;
-                        if (kc < p.kc1)
-                            tc::tma_load_4d(&mapA0, &full[stage], dstA, kc * BK, x0, y0, tb * p.bb);
-                        else
-                            tc::tma_load_4d(&mapA1, &full[stage], dstA, (kc - p.kc1) * BK, x0, y0, tb * p.bb);
-                        if (!BRES) tc::tma_load_4d(&mapB, &full[stage], dstB, kb * BK, n0, 0, 0);
-                    }
+                    const int kct = p.kc1 + p.kc2;
+                    const int tap = kb / kct, kc = kb - tap * kct;
+                    const int dy = tap / p.tap_w, dx = tap - dy * p.tap_w;
+                    const int x0 = tx * p.bw * p.stride + dx - p.pad + p.off_x;
+                    const int y0 = ty * p.bh * p.stride + dy - p.pad + p.off_y;
+                    if (kc < p.kc1)
+                        tc::tma_load_4d(&mapA0, &full[stage], dstA, kc * BK, x0, y0, tb * p.bb);
+                    else
+                        tc::tma_load_4d(&mapA1, &full[stage], dstA, (kc - p.kc1) * BK, x0, y0, tb * p.bb);
+                    if (!BRES) tc::tma_load_4d(&mapB, &full[stage], dstB, kb * BK, n_blk * BN, 0, 0);
                 }
-              }
             }
         }
-    } else if (warp == 1 && lane == 0 && rank == 0) {
-        // ------------------------------------------------------------ MMA issuer (PAIR: the leader CTA only)
-        constexpr uint32_t idesc = tc::make_idesc_f16(PAIR ? 2 * BM : BM, UN);
-        int it = 0, lt = 0;
-        if constexpr (BRES) {
-            tc::mbar_wait(b_full, 0);
-            tc::fence_after_sync();
-        }
-        for (int unit = unit0; unit < n_units; unit += unit_step, ++lt) {
-            const int sp = BRES ? 0 : unit % p.splits;
-            const int kb0 = sp * p.kb_per_split, kb1 = min(p.num_kb, kb0 + p.kb_per_split);
-            const int acc = lt % NBUF, use = lt / NBUF;
-            if (use >= 1) {                                  // the epilogue must have drained this accumulator
-                tc::mbar_wait(&tmem_empty[acc], (use - 1) & 1);
-                tc::fence_after_sync();
-            }
-            const uint32_t d_tmem = tmem_base + acc * ACC_COLS;
-            for (int kbs = kb0; kbs < kb1; kbs += SLABS, ++it) {
-                const int stage = it % STAGES;
-                const uint32_t phase = (it / STAGES) & 1;
-                const int nsl = min(SLABS, kb1 - kbs);
-                tc::mbar_wait(&full[stage], phase);
-                tc::fence_after_sync();
-              for (int sl = 0; sl < nsl; ++sl) {
-                const int kb = kbs + sl;
-                const uint32_t a_base = tc::smem_u32(sA + (stage * SLABS + sl) * A_TILE_BYTES);
-                const uint32_t b_base = tc::smem_u32(sB + (BRES ? kb : stage * SLABS + sl) * B_TILE_BYTES);
-#pragma unroll
-                for (int k = 0; k < BK / 16; ++k) {
-                    const uint64_t da = tc::make_desc_sw128(a_base + k * 32);
-#pragma unroll
-                    for (int i = 0; i < NI; ++i) {
-                        const uint64_t db = tc::make_desc_sw128(b_base + i * (UN / 2) * BK * 2 + k * 32);
-                        if constexpr (PAIR) tc::mma_f16_pair(d_tmem + i * UN, da, db, idesc, ((kb - kb0) | k) ? 1u : 0u);
-                        else tc::mma_f16(d_tmem + i * UN, da, db, idesc, ((kb - kb0) | k) ? 1u : 0u);
-                    }
-                }
-              }
-                if constexpr (PAIR) tc::mma_commit_pair(&empty[stage]);
-                else tc::mma_commit(&empty[stage]);
-            }
-            if constexpr (PAIR) tc::mma_commit_pair(&tmem_full[acc]);
-            else tc::mma_commit(&tmem_full[acc]);
-        }
-    } else if (warp >= 2) {
-        // ------------------------------------------------------------ epilogue (EPI_SETS x 4 warps)
-        // warp w reads TMEM lanes [32*(w%4), +32) (hardware restriction) and the column half (w-2)/4 of the tile.
-        const int q = warp & 3;
-        const int half_id = (warp - 2) >> 2;
-        const int row = q * 32 + lane;      // row of the 128-row tile == TMEM lane
-        // 64 bytes (one 32-column run of fp16 side input): two 256-bit loads when 32-byte aligned, else four 128-bit
-        auto ld64 = [](const __half* src, uint4* q4) {
-            if ((reinterpret_cast<uintptr_t>(src) & 31) == 0) {
-                tc::ld_global_256(src, q4[0], q4[1]);
-                tc::ld_global_256(src + 16, q4[2], q4[3]);
-            } else {
-                const uint4* s4 = reinterpret_cast<const uint4*>(src);
-#pragma unroll
-                for (int j = 0; j < 4; ++j) q4[j] = s4[j];
-            }
-        };
-        int lt = 0;
-        const uint32_t tmem_empty_leader = PAIR ? tc::mapa_u32(tc::smem_u32(&tmem_empty[0]), 0) : 0;
-        for (int unit = unit0; unit < n_units; unit += unit_step, ++lt) {
-            const int tile = BRES ? unit * p.tiles_n + nb_fixed : unit / p.splits, sp = BRES ? 0 : unit - (unit / p.splits) * p.splits;
-            const int acc = lt % NBUF;
-            const int z = tile / tiles_mn, mn = tile - z * tiles_mn;
-            const int m_row = mn / p.tiles_n, n_blk = mn - m_row * p.tiles_n;
-            const int m_blk = PAIR ? 2 * m_row + rank : m_row;
-            const int b1 = z % p.batch1, b2 = z / p.batch1;
-            bool row_ok;
-            long out_off, res_off;
-            int img = 0;
-            if (!p.conv) {
-                const int m = m_blk * BM + row;
-                row_ok = m < p.M;
-                out_off = static_cast<long>(b2) * p.so2 + static_cast<long>(b1) * p.so1 + static_cast<long>(m) * p.ldo;
-                res_off = static_cast<long>(b2) * p.sr2 + static_cast<long>(b1) * p.sr1 + static_cast<long>(m) * p.ldr;
-            } else {
-                const int tx = m_blk % p.tiles_x, ty = (m_blk / p.tiles_x) % p.tiles_y, tb = m_blk / (p.tiles_x * p.tiles_y);
-                const int xi = row % p.bw, yi = (row / p.bw) % p.bh, bi = row / (p.bw * p.bh);
-                const int x = tx * p.bw + xi, y = ty * p.bh + yi;
-                img = tb * p.bb + bi;
-                row_ok = (x < p.Wo) && (y < p.Ho) && (img < p.Bn);
-                const long pix = (static_cast<long>(img) * p.HoF + (y * p.osy + p.ooy)) * p.WoF + (x * p.osx + p.oox);
-                out_off = pix * p.ldo;
-                res_off = pix * p.ldr;
-            }
-            const int m_glob = m_blk * BM + row;
-            const float bias_row = (p.bias_mode == 2 && row_ok) ? __half2float(p.bias[m_glob]) : 0.f;
-            tc::mbar_wait(&tmem_full[acc], (lt / NBUF) & 1);
-            tc::fence_after_sync();
-#pragma unroll 1
-            for (int c0 = half_id * 32; c0 < BN; c0 += 32 * EPI_SETS) {   // the warp sets take the 32-column runs round-robin
-                uint32_t v[32];
-                tc::tmem_ld_32x32(tmem_base + acc * ACC_COLS + (static_cast<uint32_t>(q * 32) << 16) + c0, v);
-                tc::tmem_wait_ld();
-                const int n0 = n_blk * BN + c0;
-                if (!row_ok || n0 >= p.N) continue;
-                if (p.splits > 1) {   // raw partial sums; ws rows are dense with pitch N in output-row order
-                    float* wp = p.ws + sp * p.ws_split_stride + (out_off / p.ldo) * p.N + n0;
-                    if (n0 + 32 <= p.N && (p.N & 3) == 0) {
-#pragma unroll
-                        for (int i = 0; i < 8; ++i)
-                            reinterpret_cast<uint4*>(wp)[i] = make_uint4(v[4 * i], v[4 * i + 1], v[4 * i + 2], v[4 * i + 3]);
-                    } else {
-                        for (int i = 0; i < 32; ++i)
-                            if (n0 + i < p.N) wp[i] = __uint_as_float(v[i]);
-                    }
-                    continue;
-                }
-                float f[32];
-#pragma unroll
-                for (int i = 0; i < 32; ++i) f[i] = __uint_as_float(v[i]) * p.alpha + bias_row;
-                const bool full = n0 + 32 <= p.N;
-                // per-column bias and per-image bias: 16-byte loads when the 32-column run is complete and aligned
-                if (p.bias_mode == 1) {
-                    if (full && ((reinterpret_cast<uintptr_t>(p.bias + n0) & 15) == 0)) {
-                        uint4 q4[4];
-                        ld64(p.bias + n0, q4);
-#pragma unroll
-                        for (int j = 0; j < 4; ++j) {
-                            const uint4 bv = q4[j];
-                            const __half2* bh = reinterpret_cast<const __half2*>(&bv);
-#pragma unroll
-                            for (int e = 0; e < 4; ++e) {
-                                const float2 t = __half22float2(bh[e]);
-                                f[8 * j + 2 * e] += t.x;
-                                f[8 * j + 2 * e + 1] += t.y;
-                            }
-                        }
-                    } else {
-                        for (int i = 0; i < 32; ++i)
-                            if (n0 + i < p.N) f[i] += __half2float(p.bias[n0 + i]);
-                    }
-                }
-                if (p.bias2) {
-                    const __half* b2p = p.bias2 + static_cast<long>(img) * p.bias2_pitch + n0;
-                    if (full && ((reinterpret_cast<uintptr_t>(b2p) & 15) == 0)) {
-                        uint4 q4[4];
-                        ld64(b2p, q4);
-#pragma unroll
-                        for (int j = 0; j < 4; ++j) {
-                            const uint4 bv = q4[j];
-                            const __half2* bh = reinterpret_cast<const __half2*>(&bv);
-#pragma unroll
-                            for (int e = 0; e < 4; ++e) {
-                                const float2 t = __half22float2(bh[e]);
-                                f[8 * j + 2 * e] += t.x;
-                                f[8 * j + 2 * e + 1] += t.y;
-                            }
-                        }
-                    } else {
-                        for (int i = 0; i < 32; ++i)
-                            if (n0 + i < p.N) f[i] += __half2float(b2p[i]);
-                    }
-                }
-                if (p.act == 2) {
-                    // GEGLU: the 32-column run is [16 value | 16 gate] columns of the same 16 outputs (weight rows
-                    // interleaved by the caller); D has N/2 columns: out[n0/2 + j] = value_j * gelu(gate_j)
-                    __half* dst = p.out + out_off + (n0 >> 1);
-                    uint32_t pk[8];
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) {
-                        const float g0 = f[16 + 2 * j], g1 = f[17 + 2 * j];
-                        const float y0 = f[2 * j] * gelu_erf_fast(g0);
-                        const float y1 = f[2 * j + 1] * gelu_erf_fast(g1);
-                        const __half2 h = __floats2half2_rn(y0, y1);
-                        pk[j] = *reinterpret_cast<const uint32_t*>(&h);
-                    }
-                    if ((reinterpret_cast<uintptr_t>(dst) & 31) == 0) {
-                        tc::st_global_256(dst, make_uint4(pk[0], pk[1], pk[2], pk[3]), make_uint4(pk[4], pk[5], pk[6], pk[7]));
-                    } else {
-                        reinterpret_cast<uint4*>(dst)[0] = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-                        reinterpret_cast<uint4*>(dst)[1] = make_uint4(pk[4], pk[5], pk[6], pk[7]);
-                    }
-                    continue;
-                }
-                if (p.act) {
-#pragma unroll
-                    for (int i = 0; i < 32; ++i) f[i] = apply_act(f[i], p.act);
-                }
-                if (p.residual) {
-                    const __half* rp = p.residual + res_off + n0;
-                    if (full && ((reinterpret_cast<uintptr_t>(rp) & 15) == 0)) {
-                        uint4 q4[4];
-                        ld64(rp, q4);
-#pragma unroll
-                        for (int j = 0; j < 4; ++j) {
-                            const uint4 rv = q4[j];
-                            const __half2* rh = reinterpret_cast<const __half2*>(&rv);
-#pragma unroll
-                            for (int e = 0; e < 4; ++e) {
-                                const float2 t = __half22float2(rh[e]);
-                                f[8 * j + 2 * e] += t.x;
-                                f[8 * j + 2 * e + 1] += t.y;
-                            }
-                        }
-                    } else {
-                        for (int i = 0; i < 32; ++i)
-                            if (n0 + i < p.N) f[i] += __half2float(rp[i]);
-                    }
-                }
-                if (p.out_f32) {
-                    for (int i = 0; i < 32; ++i)
-                        if (n0 + i < p.N) p.out_f32[out_off + n0 + i] = f[i];
-                } else if (full && ((reinterpret_cast<uintptr_t>(p.out + out_off + n0) & 15) == 0)) {
-                    uint4* dst = reinterpret_cast<uint4*>(p.out + out_off + n0);
-                    uint4 pk[4];
-#pragma unroll
-                    for (int i = 0; i < 4; ++i) {
-                        __half2 h0 = __floats2half2_rn(f[8 * i + 0], f[8 * i + 1]);
-                        __half2 h1 = __floats2half2_rn(f[8 * i + 2], f[8 * i + 3]);
-                        __half2 h2 = __floats2half2_rn(f[8 * i + 4], f[8 * i + 5]);
-                        __half2 h3 = __floats2half2_rn(f[8 * i + 6], f[8 * i + 7]);
-                        pk[i].x = *reinterpret_cast<uint32_t*>(&h0);
-                        pk[i].y = *reinterpret_cast<uint32_t*>(&h1);
-                        pk[i].z = *reinterpret_cast<uint32_t*>(&h2);
-                        pk[i].w = *reinterpret_cast<uint32_t*>(&h3);
-                    }
-                    if ((reinterpret_cast<uintptr_t>(dst) & 31) == 0) {   // whole 32-byte sectors per store
-                        tc::st_global_256(dst, pk[0], pk[1]);
-                        tc::st_global_256(dst + 2, pk[2], pk[3]);
-                    } else {
-#pragma unroll
-                        for (int i = 0; i < 4; ++i) dst[i] = pk[i];
-                    }
-                } else {
-                    for (int i = 0; i < 32; ++i)
-                        if (n0 + i < p.N) p.out[out_off + n0 + i] = __float2half_rn(f[i]);
-                }
-            }
-            tc::fence_before_sync();
-            __syncwarp();
-            if (lane == 0) {   // one arrival per epilogue warp: the accumulator may be overwritten
-                if constexpr (PAIR) tc::mbar_arrive_cluster(tmem_empty_leader + acc * 8);
-                else tc::mbar_arrive(&tmem_empty[acc]);
-            }
-        }
+        return;
     }
-    tc::fence_before_sync();
-    if constexpr (PAIR) tc::cluster_sync_all();   // the leader's MMAs read the peer's shared memory until the very end
-    else __syncthreads();
-    if (warp == 1) {
-        tc::fence_after_sync();
-        if constexpr (PAIR) tc::tmem_dealloc_pair(tmem_base, NBUF * ACC_COLS);
-        else tc::tmem_dealloc(tmem_base, NBUF * ACC_COLS);
+
+    // ---------------------------------------------------------------- consumers (threads 0-255)
+    const int wg = warp >> 2;                    // rows [64 wg, +64) of the tile
+    const int frag_row = wg * 64 + (warp & 3) * 16 + (lane >> 2), frag_col = 2 * (lane & 3);
+    const int row = threadIdx.x & 127;           // epilogue: one tile row per thread, two threads per row
+    const int half_id = threadIdx.x >> 7;
+    // 64 bytes (one 32-column run of fp16 side input) as four 128-bit loads
+    auto ld64 = [](const __half* src, uint4* q4) {
+        const uint4* s4 = reinterpret_cast<const uint4*>(src);
+#pragma unroll
+        for (int j = 0; j < 4; ++j) q4[j] = s4[j];
+    };
+    if constexpr (BRES) tc::mbar_wait(b_full, 0);
+    int it = 0;
+    for (int unit = unit0; unit < n_units; unit += unit_step) {
+        const int tile = BRES ? unit * p.tiles_n + nb_fixed : unit / p.splits, sp = BRES ? 0 : unit - (unit / p.splits) * p.splits;
+        const int kb0 = sp * p.kb_per_split, kb1 = min(p.num_kb, kb0 + p.kb_per_split);
+        // ---- main loop: one wgmma group per stage, at most one group in flight behind the newest
+        float acc[BN / 2];
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+        int prev = -1;
+        for (int kb = kb0; kb < kb1; ++kb, ++it) {
+            const int stage = it % STAGES;
+            tc::mbar_wait(&full[stage], (it / STAGES) & 1);
+            const uint32_t a_base = tc::smem_u32(sA + stage * A_TILE_BYTES) + wg * (64 * 128);
+            const uint32_t b_base = tc::smem_u32(sB + (BRES ? kb : stage) * B_TILE_BYTES);
+            tc::wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < BK / 16; ++k)
+                tc::wgmma_ss<BN>(acc, tc::make_desc_sw128(a_base + k * 32), tc::make_desc_sw128(b_base + k * 32), 1u);
+            tc::wgmma_commit();
+            tc::wgmma_wait<1>();                 // the group of the previous stage has completed: release that stage
+            tc::reg_fence<BN / 2>(acc);
+            if (prev >= 0) tc::mbar_arrive(&empty[prev]);
+            prev = stage;
+        }
+        tc::wgmma_wait<0>();
+        tc::reg_fence<BN / 2>(acc);
+        if (prev >= 0) tc::mbar_arrive(&empty[prev]);
+
+        // ---- accumulators -> fp32 staging tile (the previous unit's epilogue must be done reading it)
+        named_bar_sync(1, 256);
+#pragma unroll
+        for (int i = 0; i < BN / 8; ++i) {
+            const int c = 8 * i + frag_col;
+            *reinterpret_cast<float2*>(stg + frag_row * PITCH + c) = make_float2(acc[4 * i], acc[4 * i + 1]);
+            *reinterpret_cast<float2*>(stg + (frag_row + 8) * PITCH + c) = make_float2(acc[4 * i + 2], acc[4 * i + 3]);
+        }
+        named_bar_sync(1, 256);
+
+        // ---- epilogue: thread (row, half_id) takes the 32-column runs half_id, half_id + 2, ... of its row
+        const int z = tile / tiles_mn, mn = tile - z * tiles_mn;
+        const int m_blk = mn / p.tiles_n, n_blk = mn - m_blk * p.tiles_n;
+        const int b1 = z % p.batch1, b2 = z / p.batch1;
+        bool row_ok;
+        long out_off, res_off;
+        int img = 0;
+        if (!p.conv) {
+            const int m = m_blk * BM + row;
+            row_ok = m < p.M;
+            out_off = static_cast<long>(b2) * p.so2 + static_cast<long>(b1) * p.so1 + static_cast<long>(m) * p.ldo;
+            res_off = static_cast<long>(b2) * p.sr2 + static_cast<long>(b1) * p.sr1 + static_cast<long>(m) * p.ldr;
+        } else {
+            const int tx = m_blk % p.tiles_x, ty = (m_blk / p.tiles_x) % p.tiles_y, tb = m_blk / (p.tiles_x * p.tiles_y);
+            const int xi = row % p.bw, yi = (row / p.bw) % p.bh, bi = row / (p.bw * p.bh);
+            const int x = tx * p.bw + xi, y = ty * p.bh + yi;
+            img = tb * p.bb + bi;
+            row_ok = (x < p.Wo) && (y < p.Ho) && (img < p.Bn);
+            const long pix = (static_cast<long>(img) * p.HoF + (y * p.osy + p.ooy)) * p.WoF + (x * p.osx + p.oox);
+            out_off = pix * p.ldo;
+            res_off = pix * p.ldr;
+        }
+        const int m_glob = m_blk * BM + row;
+        const float bias_row = (p.bias_mode == 2 && row_ok) ? __half2float(p.bias[m_glob]) : 0.f;
+#pragma unroll 1
+        for (int c0 = half_id * 32; c0 < BN; c0 += 64) {
+            const int n0 = n_blk * BN + c0;
+            if (!row_ok || n0 >= p.N) continue;
+            float f[32];
+#pragma unroll
+            for (int i = 0; i < 8; ++i) {
+                const float4 t = *reinterpret_cast<const float4*>(stg + row * PITCH + c0 + 4 * i);
+                f[4 * i] = t.x; f[4 * i + 1] = t.y; f[4 * i + 2] = t.z; f[4 * i + 3] = t.w;
+            }
+            if (p.splits > 1) {   // raw partial sums; ws rows are dense with pitch N in output-row order
+                float* wp = p.ws + sp * p.ws_split_stride + (out_off / p.ldo) * p.N + n0;
+                if (n0 + 32 <= p.N && (p.N & 3) == 0) {
+#pragma unroll
+                    for (int i = 0; i < 8; ++i)
+                        reinterpret_cast<float4*>(wp)[i] = make_float4(f[4 * i], f[4 * i + 1], f[4 * i + 2], f[4 * i + 3]);
+                } else {
+                    for (int i = 0; i < 32; ++i)
+                        if (n0 + i < p.N) wp[i] = f[i];
+                }
+                continue;
+            }
+#pragma unroll
+            for (int i = 0; i < 32; ++i) f[i] = f[i] * p.alpha + bias_row;
+            const bool full_run = n0 + 32 <= p.N;
+            // per-column bias and per-image bias: 16-byte loads when the 32-column run is complete and aligned
+            if (p.bias_mode == 1) {
+                if (full_run && ((reinterpret_cast<uintptr_t>(p.bias + n0) & 15) == 0)) {
+                    uint4 q4[4];
+                    ld64(p.bias + n0, q4);
+#pragma unroll
+                    for (int j = 0; j < 4; ++j) {
+                        const uint4 bv = q4[j];
+                        const __half2* bh = reinterpret_cast<const __half2*>(&bv);
+#pragma unroll
+                        for (int e = 0; e < 4; ++e) {
+                            const float2 t = __half22float2(bh[e]);
+                            f[8 * j + 2 * e] += t.x;
+                            f[8 * j + 2 * e + 1] += t.y;
+                        }
+                    }
+                } else {
+                    for (int i = 0; i < 32; ++i)
+                        if (n0 + i < p.N) f[i] += __half2float(p.bias[n0 + i]);
+                }
+            }
+            if (p.bias2) {
+                const __half* b2p = p.bias2 + static_cast<long>(img) * p.bias2_pitch + n0;
+                if (full_run && ((reinterpret_cast<uintptr_t>(b2p) & 15) == 0)) {
+                    uint4 q4[4];
+                    ld64(b2p, q4);
+#pragma unroll
+                    for (int j = 0; j < 4; ++j) {
+                        const uint4 bv = q4[j];
+                        const __half2* bh = reinterpret_cast<const __half2*>(&bv);
+#pragma unroll
+                        for (int e = 0; e < 4; ++e) {
+                            const float2 t = __half22float2(bh[e]);
+                            f[8 * j + 2 * e] += t.x;
+                            f[8 * j + 2 * e + 1] += t.y;
+                        }
+                    }
+                } else {
+                    for (int i = 0; i < 32; ++i)
+                        if (n0 + i < p.N) f[i] += __half2float(b2p[i]);
+                }
+            }
+            if (p.act == 2) {
+                // GEGLU: the 32-column run is [16 value | 16 gate] columns of the same 16 outputs (weight rows
+                // interleaved by the caller); D has N/2 columns: out[n0/2 + j] = value_j * gelu(gate_j)
+                __half* dst = p.out + out_off + (n0 >> 1);
+                uint32_t pk[8];
+#pragma unroll
+                for (int j = 0; j < 8; ++j) {
+                    const float g0 = f[16 + 2 * j], g1 = f[17 + 2 * j];
+                    const float y0 = f[2 * j] * gelu_erf_fast(g0);
+                    const float y1 = f[2 * j + 1] * gelu_erf_fast(g1);
+                    const __half2 h = __floats2half2_rn(y0, y1);
+                    pk[j] = *reinterpret_cast<const uint32_t*>(&h);
+                }
+                reinterpret_cast<uint4*>(dst)[0] = make_uint4(pk[0], pk[1], pk[2], pk[3]);
+                reinterpret_cast<uint4*>(dst)[1] = make_uint4(pk[4], pk[5], pk[6], pk[7]);
+                continue;
+            }
+            if (p.act) {
+#pragma unroll
+                for (int i = 0; i < 32; ++i) f[i] = apply_act(f[i], p.act);
+            }
+            if (p.residual) {
+                const __half* rp = p.residual + res_off + n0;
+                if (full_run && ((reinterpret_cast<uintptr_t>(rp) & 15) == 0)) {
+                    uint4 q4[4];
+                    ld64(rp, q4);
+#pragma unroll
+                    for (int j = 0; j < 4; ++j) {
+                        const uint4 rv = q4[j];
+                        const __half2* rh = reinterpret_cast<const __half2*>(&rv);
+#pragma unroll
+                        for (int e = 0; e < 4; ++e) {
+                            const float2 t = __half22float2(rh[e]);
+                            f[8 * j + 2 * e] += t.x;
+                            f[8 * j + 2 * e + 1] += t.y;
+                        }
+                    }
+                } else {
+                    for (int i = 0; i < 32; ++i)
+                        if (n0 + i < p.N) f[i] += __half2float(rp[i]);
+                }
+            }
+            if (p.out_f32) {
+                for (int i = 0; i < 32; ++i)
+                    if (n0 + i < p.N) p.out_f32[out_off + n0 + i] = f[i];
+            } else if (full_run && ((reinterpret_cast<uintptr_t>(p.out + out_off + n0) & 15) == 0)) {
+                uint4* dst = reinterpret_cast<uint4*>(p.out + out_off + n0);
+#pragma unroll
+                for (int i = 0; i < 4; ++i) {
+                    __half2 h0 = __floats2half2_rn(f[8 * i + 0], f[8 * i + 1]);
+                    __half2 h1 = __floats2half2_rn(f[8 * i + 2], f[8 * i + 3]);
+                    __half2 h2 = __floats2half2_rn(f[8 * i + 4], f[8 * i + 5]);
+                    __half2 h3 = __floats2half2_rn(f[8 * i + 6], f[8 * i + 7]);
+                    dst[i] = make_uint4(*reinterpret_cast<uint32_t*>(&h0), *reinterpret_cast<uint32_t*>(&h1),
+                                        *reinterpret_cast<uint32_t*>(&h2), *reinterpret_cast<uint32_t*>(&h3));
+                }
+            } else {
+                for (int i = 0; i < 32; ++i)
+                    if (n0 + i < p.N) p.out[out_off + n0 + i] = __float2half_rn(f[i]);
+            }
+        }
     }
 }
 
@@ -571,32 +457,34 @@ struct TcProfile {
     struct Rec { int conv, M, N, K, batch, splits, bn; };   // bn < 0: CTA-pair kernel
     std::vector<Rec> recs;
 };
+int num_sms_cached() {
+    static int n = 0;
+    if (!n) {
+        int dev = 0;
+        if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess)
+            n = 132;
+    }
+    return n;
+}
+
 TcProfile g_prof;
 std::mutex g_prof_mu;
 
-template <int BN, int STAGES, bool PAIR, int SLABS, bool BRES = false>
+template <int BN, int STAGES, bool BRES = false>
 int launch(const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& b, const TcParams& p, dim3 grid,
            cudaStream_t st) {   // `grid` arrives as (tiles_n, tiles_m, batch) and is flattened to a persistent 1-D grid
-    constexpr size_t smem = static_cast<size_t>(STAGES) * SLABS * A_TILE_BYTES +
-                            static_cast<size_t>(BRES ? BRES_KB : STAGES * SLABS) * ((PAIR ? BN / 2 : BN) * BK * 2) + 1024;
-    static_assert(smem <= 232448, "shared memory budget");
-    static int num_sms = 0;
-    if (!num_sms) {
-        int dev = 0;
-        RF_CUDA_TRY(cudaGetDevice(&dev));
-        RF_CUDA_TRY(cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev));
-    }
+    constexpr size_t smem = static_cast<size_t>(STAGES) * A_TILE_BYTES +
+                            static_cast<size_t>(BRES ? BRES_KB : STAGES) * (BN * BK * 2) + stage_bytes(BN) + 1024;
+    static_assert(smem <= 232448, "shared memory budget (227 KB per block)");
+    const int num_sms = num_sms_cached();
     const int n_tiles = static_cast<int>(grid.x * grid.y * grid.z);
-    if (PAIR) {   // one CTA pair per TPC
-        const int pairs = num_sms / 2;
-        grid = dim3(static_cast<unsigned>(2 * (n_tiles < pairs ? n_tiles : pairs)));
-    } else if (BRES) {   // every CTA is bound to one column block: a multiple of tiles_n CTAs
+    if (BRES) {   // every CTA is bound to one column block: a multiple of tiles_n CTAs
         grid = dim3(static_cast<unsigned>((num_sms / p.tiles_n) * p.tiles_n));
     } else {
         grid = dim3(static_cast<unsigned>(n_tiles < num_sms ? n_tiles : num_sms));
     }
     static rf_dev_once once;
-    const cudaError_t aerr = rf_set_smem_once(once, k_tc_gemm<BN, STAGES, PAIR, SLABS, BRES>, int(smem));
+    const cudaError_t aerr = rf_set_smem_once(once, k_tc_gemm<BN, STAGES, BRES>, int(smem));
     if (aerr != cudaSuccess) return rf_fail(RF_ERR_CUDA, std::string("cudaFuncSetAttribute: ") + cudaGetErrorString(aerr));
     cudaEvent_t e0 = nullptr, e1 = nullptr;
     const bool prof = g_prof.on;
@@ -605,17 +493,8 @@ int launch(const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& b, c
         RF_CUDA_TRY(cudaEventCreate(&e1));
         RF_CUDA_TRY(cudaEventRecord(e0, st));
     }
-    {
-        cudaLaunchAttribute attr[2];
-        if (PAIR) {
-            attr[0].id = cudaLaunchAttributeClusterDimension;
-            attr[0].val.clusterDim.x = 2;
-            attr[0].val.clusterDim.y = 1;
-            attr[0].val.clusterDim.z = 1;
-        }
-        RF_LAUNCH_PDL_ATTRS("k_tc_gemm", (k_tc_gemm<BN, STAGES, PAIR, SLABS, BRES>), grid, dim3(GEMM_THREADS), smem, st,
-                            n_tiles <= 2 * num_sms, attr, PAIR ? 1 : 0, a0, a1, b, p);
-    }
+    RF_LAUNCH_PDL("k_tc_gemm", (k_tc_gemm<BN, STAGES, BRES>), grid, dim3(GEMM_THREADS), smem, st, n_tiles <= 2 * num_sms,
+                  a0, a1, b, p);
     if (prof) {
         RF_CUDA_TRY(cudaEventRecord(e1, st));
         std::lock_guard<std::mutex> lk(g_prof_mu);
@@ -625,7 +504,7 @@ int launch(const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& b, c
         const double m = p.conv ? static_cast<double>(p.Bn) * p.Ho * p.Wo : static_cast<double>(p.M) * p.batch1 * p.batch2;
         g_prof.flops += 2.0 * m * p.N * p.K;
         g_prof.recs.push_back({p.conv, p.conv ? p.Bn * p.Ho * p.Wo : p.M, p.N, p.K, p.batch1 * p.batch2, p.splits,
-                               PAIR ? -BN : (BRES ? 1000 + BN : BN)});
+                               BRES ? 1000 + BN : BN});
     }
     return RF_OK;
 }
@@ -705,109 +584,25 @@ int pick_splits(long rows, int N, int tiles, int num_kb, int num_sms, bool allow
 
 // Output-tile width: 64 for narrow outputs; otherwise 128, or 160 when it divides N and is not slower by the wave
 // count: relative time = ceil(tiles / SMs) waves x tile width.  160 always wins when 128 does not divide N (N = 320:
-// two exact tiles instead of three with 17 % padding) and often when both do (M = 4096, N = 1280: 256 tiles = 2 waves
-// instead of 320 tiles = 3 waves); it also moves 12 % fewer operand bytes per FLOP from L2.
+// two exact tiles instead of three with 17 % padding) and often when both do; it also moves 12 % fewer operand bytes
+// per FLOP from L2.  RF_GEMM_BN=<64|128|160> forces a width where it is legal (A/B measurements, parity tests).
 int pick_bn(int N, long tiles_m) {
+    if (const char* env = getenv("RF_GEMM_BN")) {        // read per call: the parity tests flip it inside one process
+        const int bn = atoi(env);
+        if (bn == 64 || bn == 128 || (bn == 160 && N % 160 == 0)) return bn;
+    }
     if (N <= 64) return 64;
     if (N % 160) return 128;
-    const long sms = 148;
+    const long sms = num_sms_cached();
     const long t128 = tiles_m * ((N + 127) / 128), t160 = tiles_m * (N / 160);
     const long c128 = ((t128 + sms - 1) / sms) * 128, c160 = ((t160 + sms - 1) / sms) * 160;
     return c160 * 100 <= c128 * 102 ? 160 : 128;
 }
 
-int num_sms_cached() {
-    static int n = 0;
-    if (!n) {
-        int dev = 0;
-        if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess)
-            n = 148;
-    }
-    return n;
-}
-
-// Tile configuration of one problem: width BN and whether the CTA-pair kernel (256 x BN tiles, cta_group::2) runs it.
-// Measured (profiles/r02_tile_configs.md): pairs pay off with 256-wide tiles only — 1.25-1.30x the 1-SM kernel on the
-// N = 1280 / 2560 / 5120 / 10240 layers (up to 1460 TFLOP/s) — while pair tiles of 160 / 128 columns are no faster than
-// the 1-SM kernel.  So: pair + BN 256 when 256 divides N (or N == 256), the problem fills two waves, and the padding of
-// odd row-block counts (per batch entry) does not eat the gain; otherwise the 1-SM kernel with pick_bn's width.
-// RF_GEMM_PAIR=0 disables pairs, RF_GEMM_BN=<256|160|128> forces a pair tile width (A/B measurements, parity tests).
-struct TileCfg {
-    int bn;
-    bool pair;
-};
-TileCfg pick_cfg(int N, long tiles_m, int nbatch, int num_kb) {
-    const char* env_pair = getenv("RF_GEMM_PAIR");      // read per call: the parity tests flip them inside one process
-    const char* env_bn = getenv("RF_GEMM_BN");
-    const long tiles_m_total = tiles_m * nbatch;
-    TileCfg c{pick_bn(N, tiles_m_total), false};
-    if ((env_pair && env_pair[0] == '0') || N < 128) return c;
-    const long sms = num_sms_cached(), pairs = sms / 2;
-    const long rows2 = ((tiles_m + 1) / 2) * nbatch;
-    if (env_bn) {                                        // forced pair width
-        const int bn = atoi(env_bn);
-        if ((bn == 320 || bn == 256 || bn == 160 || bn == 128) && !(bn == 160 && N % 160) && !(bn == 320 && N % 320) &&
-            tiles_m_total * ((N + c.bn - 1) / c.bn) >= 2 * sms) {
-            c.bn = bn;
-            c.pair = true;
-        }
-        return c;
-    }
-    if ((N % 256) != 0) {
-        // N = 320 / 640 / 960 ...: 320-wide pair tiles (two instructions, no accumulator double buffering) when K is long
-        // enough to amortise the exposed epilogue (~4000 clk per tile against 640 clk per K slab).  Measured at batch 64
-        // (profiles/r02_tile_configs.md): K >= 2880 (every 3x3 conv) gains 5-30 % (up to 1450 TFLOP/s), K = 1920-2560 is
-        // even, K <= 1280 loses 10-25 % against the 1-SM 128 x 160 tile -> threshold 45 slabs.
-        const char* env320 = getenv("RF_GEMM_320_MIN_KB");
-        const int min_kb = env320 ? atoi(env320) : 45;
-        if ((N % 320) == 0 && num_kb >= min_kb && tiles_m_total * (N / 160) >= 2 * sms) {
-            c.bn = 320;
-            c.pair = true;
-        }
-        return c;
-    }
-    const long t1 = tiles_m_total * ((N + c.bn - 1) / c.bn), t2 = rows2 * (N / 256);
-    if (t1 < 2 * sms) return c;
-    const double cost1 = static_cast<double>((t1 + sms - 1) / sms) * c.bn;
-    const double cost2 = static_cast<double>((t2 + pairs - 1) / pairs) * 256 / 1.25;
-    if (cost2 < cost1) {
-        c.bn = 256;
-        c.pair = true;
-    }
-    return c;
-}
-
-// rows of B one TMA load brings in: the whole tile (1-SM), this CTA's half (pairs), half of one 160-wide instruction (BN 320)
-int b_box_rows(const TileCfg& c) { return !c.pair ? c.bn : (c.bn == 320 ? 80 : c.bn / 2); }
-
-int dispatch(int N, const TileCfg cfg, const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& b, TcParams& p,
+int dispatch(int N, int bn, const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& b, TcParams& p,
              int tiles_m, int nbatch, cudaStream_t st, void* ws, size_t ws_bytes, size_t* query) {
-    // one persistent CTA (or CTA pair) per SM (TPC): TMA ring of 3-4 stages x 2 K slabs, 2 TMEM accumulators
-    const int bn = cfg.bn;
-    const char* env_slabs = getenv("RF_GEMM_SLABS");          // A/B: 1 = one slab per stage (round-1 ring), 3 = three (BN 160)
-    const int slabs = env_slabs ? atoi(env_slabs) : 2;
+    // one persistent CTA per SM: TMA ring of 3-6 stages of one 64-wide K slab each (as many as fit next to the staging tile)
     p.tiles_n = (N + bn - 1) / bn;
-    if (cfg.pair) {
-        if (query) {
-            *query = 0;
-            return RF_OK;
-        }
-        p.tiles_m = (tiles_m + 1) / 2;          // 256-row blocks
-        p.splits = 1;
-        p.kb_per_split = p.num_kb;
-        p.ws = nullptr;
-        dim3 grid(p.tiles_n, p.tiles_m, nbatch);
-        if (slabs == 1) {
-            if (bn == 320) return launch<320, 6, true, 1>(a0, a1, b, p, grid, st);
-            if (bn == 256) return launch<256, 6, true, 1>(a0, a1, b, p, grid, st);
-            if (bn == 160) return launch<160, 8, true, 1>(a0, a1, b, p, grid, st);
-            return launch<128, 8, true, 1>(a0, a1, b, p, grid, st);
-        }
-        if (bn == 320) return launch<320, 3, true, 2>(a0, a1, b, p, grid, st);
-        if (bn == 256) return launch<256, 3, true, 2>(a0, a1, b, p, grid, st);
-        if (bn == 160) return launch<160, 4, true, 2>(a0, a1, b, p, grid, st);
-        return launch<128, 4, true, 2>(a0, a1, b, p, grid, st);
-    }
     p.tiles_m = tiles_m;
     // split-K: non-batched, plain or SiLU epilogue, 16-byte aligned fp16/fp32 rows
     const long rows = p.conv ? static_cast<long>(p.Bn) * p.Ho * p.Wo : p.M;
@@ -840,19 +635,11 @@ int dispatch(int N, const TileCfg cfg, const CUtensorMap& a0, const CUtensorMap&
     const char* env_bres = getenv("RF_GEMM_BRES");
     if (bn == 160 && nbatch == 1 && p.splits == 1 && p.num_kb <= BRES_KB && p.tiles_n <= 8 &&
         static_cast<long>(tiles_m) * p.tiles_n >= 4L * num_sms_cached() && !(env_bres && env_bres[0] == '0')) {
-        return launch<160, 3, false, 2, true>(a0, a1, b, p, grid, st);       // B-stationary (K <= 320, N = 160 k)
+        return launch<160, 2, true>(a0, a1, b, p, grid, st);       // B-stationary (K <= 320, N = 160 k)
     }
-    if (slabs == 1) {
-        if (bn == 160) rc = launch<160, 6, false, 1>(a0, a1, b, p, grid, st);   // N = 320-type layers: two exact 160-column tiles
-        else if (bn == 128) rc = launch<128, 6, false, 1>(a0, a1, b, p, grid, st);
-        else rc = launch<64, 8, false, 1>(a0, a1, b, p, grid, st);
-    } else if (slabs == 3 && bn == 160) {
-        rc = launch<160, 2, false, 3>(a0, a1, b, p, grid, st);
-    } else {
-        if (bn == 160) rc = launch<160, 3, false, 2>(a0, a1, b, p, grid, st);
-        else if (bn == 128) rc = launch<128, 3, false, 2>(a0, a1, b, p, grid, st);
-        else rc = launch<64, 4, false, 2>(a0, a1, b, p, grid, st);
-    }
+    if (bn == 160) rc = launch<160, 3>(a0, a1, b, p, grid, st);   // N = 320-type layers: two exact 160-column tiles
+    else if (bn == 128) rc = launch<128, 4>(a0, a1, b, p, grid, st);
+    else rc = launch<64, 6>(a0, a1, b, p, grid, st);
     if (rc || p.splits == 1) return rc;
     const long work = rows * (N / 8);
     const unsigned blocks = static_cast<unsigned>(std::min<long>((work + 255) / 256, 8L * num_sms_cached()));
@@ -886,11 +673,11 @@ static int gemm_impl(const rf_gemm_desc* d, void* stream, size_t* query) {
         int rc = make_map(&ma, d->A, dims, str, box, es);
         if (rc) return rc;
     }
-    const TileCfg cfg = pick_cfg(d->N, (d->M + BM - 1) / BM, b1 * b2, (d->K + BK - 1) / BK);
+    const int bn = pick_bn(d->N, static_cast<long>((d->M + BM - 1) / BM) * b1 * b2);
     {
         const long dims[4] = {d->K, d->N, b_m1 ? b1 : 1, b_m2 ? b2 : 1};
         const long str[4] = {1, d->ldb, b_m1 ? d->sb1 : d->ldb, b_m2 ? d->sb2 : d->ldb};
-        const int box[4] = {BK, b_box_rows(cfg), 1, 1};
+        const int box[4] = {BK, bn, 1, 1};
         const int es[4] = {1, 1, 1, 1};
         int rc = make_map(&mb, d->B, dims, str, box, es);
         if (rc) return rc;
@@ -915,7 +702,7 @@ static int gemm_impl(const rf_gemm_desc* d, void* stream, size_t* query) {
                         (reinterpret_cast<uintptr_t>(d->D) & 15)))
         return rf_fail(RF_ERR_UNSUPPORTED, "rf_gemm_f16: GEGLU epilogue needs N % 32 == 0, fp16 output with 16-byte "
                                            "aligned rows and no residual");
-    return dispatch(d->N, cfg, ma, ma, mb, p, (d->M + BM - 1) / BM, b1 * b2, static_cast<cudaStream_t>(stream), d->workspace,
+    return dispatch(d->N, bn, ma, ma, mb, p, (d->M + BM - 1) / BM, b1 * b2, static_cast<cudaStream_t>(stream), d->workspace,
                     d->workspace_bytes > 0 ? static_cast<size_t>(d->workspace_bytes) : 0, query);
 }
 
@@ -971,11 +758,11 @@ static int conv_impl(const rf_conv_desc* d, void* stream, size_t* query) {
     const int taps = d->ksize * d->ksize;
     const long Ktot = static_cast<long>(taps) * (d->C1 + C2);
     const long conv_tiles_m = static_cast<long>((Wo + bw - 1) / bw) * ((Ho + bh - 1) / bh) * ((d->B + bb - 1) / bb);
-    const TileCfg cfg = pick_cfg(d->Cout, conv_tiles_m, 1, static_cast<int>(Ktot / BK));
+    const int bn = pick_bn(d->Cout, conv_tiles_m);
     {
         const long dims[4] = {Ktot, d->Cout, 1, 1};
         const long str[4] = {1, Ktot, Ktot * d->Cout, Ktot * d->Cout};
-        const int box[4] = {BK, b_box_rows(cfg), 1, 1};
+        const int box[4] = {BK, bn, 1, 1};
         const int es[4] = {1, 1, 1, 1};
         int rc = make_map(&mb, d->w, dims, str, box, es);
         if (rc) return rc;
@@ -1007,7 +794,7 @@ static int conv_impl(const rf_conv_desc* d, void* stream, size_t* query) {
     p.act = d->act;
     void* ws = d->workspace;
     const size_t ws_bytes = d->workspace_bytes > 0 ? static_cast<size_t>(d->workspace_bytes) : 0;
-    if (!up2) return dispatch(d->Cout, cfg, m1, m2, mb, p, p.tiles_x * p.tiles_y * tiles_b, 1, static_cast<cudaStream_t>(stream), ws,
+    if (!up2) return dispatch(d->Cout, bn, m1, m2, mb, p, p.tiles_x * p.tiles_y * tiles_b, 1, static_cast<cudaStream_t>(stream), ws,
                               ws_bytes, query);
     // conv3x3(pad 1) of the nearest-2x upsampled image == four 2x2 convolutions of the input, one per output parity
     // (py, px): output (2y + py, 2x + px) reads input rows y + py - 1 + {0, 1} and columns x + px - 1 + {0, 1}; the 3x3 taps
@@ -1021,12 +808,12 @@ static int conv_impl(const rf_conv_desc* d, void* stream, size_t* query) {
         CUtensorMap mph;
         const long dims[4] = {Ktot, d->Cout, 1, 1};
         const long str[4] = {1, Ktot, Ktot * d->Cout, Ktot * d->Cout};
-        const int box[4] = {BK, b_box_rows(cfg), 1, 1};
+        const int box[4] = {BK, bn, 1, 1};
         const int es[4] = {1, 1, 1, 1};
         int rc = make_map(&mph, static_cast<const __half*>(d->w) + static_cast<long>(ph) * d->Cout * Ktot, dims, str, box, es);
         if (rc) return rc;
         TcParams q = p;
-        rc = dispatch(d->Cout, cfg, m1, m2, mph, q, p.tiles_x * p.tiles_y * tiles_b, 1, static_cast<cudaStream_t>(stream), nullptr, 0,
+        rc = dispatch(d->Cout, bn, m1, m2, mph, q, p.tiles_x * p.tiles_y * tiles_b, 1, static_cast<cudaStream_t>(stream), nullptr, 0,
                       query);      // strided outputs: never split
         if (rc || query) return rc;
     }
@@ -1057,7 +844,7 @@ extern "C" int rf_tc_profile_end(double* ms_out, double* flops_out, long* launch
     double ms = 0.0;
     cudaError_t err = cudaDeviceSynchronize();
     FILE* dump = nullptr;
-    if (const char* path = getenv("RF_TC_PROFILE_DUMP")) dump = fopen(path, "w");   // per-launch csv for profiles/
+    if (const char* path = getenv("RF_TC_PROFILE_DUMP")) dump = fopen(path, "w");   // per-launch csv (A/B measurements)
     if (dump) fprintf(dump, "conv,M,N,K,batch,splits,bn,ms\n");
     for (size_t i = 0; i + 1 < g_prof.ev.size() && err == cudaSuccess; i += 2) {
         float t = 0.f;

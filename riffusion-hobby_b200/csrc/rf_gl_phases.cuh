@@ -105,7 +105,7 @@ RF_HD void rf_pass_a(int tid, int nt, rf_c32* V) {
 // DFT) then column phase: transposed spectral order in, natural time order out.  One thread per transform (the previous
 // form) kept 49 complex values = 98 registers live and left 166 of 256 threads idle for NA = 5.
 #ifndef RF_GL_PASS7
-#define RF_GL_PASS7 1       // 0: the one-thread-per-transform radix-49 pass (A/B builds, scratch/variants)
+#define RF_GL_PASS7 1       // 0: the one-thread-per-transform radix-49 pass (A/B builds)
 #endif
 template <bool INV, int NA, int STEP>
 RF_HD void rf_pass_c7(int tid, int nt, rf_c32* V) {

@@ -1,6 +1,5 @@
-// sm_100a tensor-core plumbing: mbarrier, TMA (cp.async.bulk.tensor), TMEM allocation,
-// tcgen05.mma / commit / ld, and the shared-memory + instruction descriptors.
-// Bit layouts follow cute/arch/mma_sm100_desc.hpp (UMMA::SmemDescriptor / InstrDescriptor).
+// sm_90a tensor-core plumbing: mbarrier, TMA (cp.async.bulk.tensor), warpgroup MMA (wgmma) and its shared-memory
+// matrix descriptors.  Descriptor bit layout: PTX ISA, "Matrix Descriptor Format" of the asynchronous warpgroup MMA.
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -41,29 +40,7 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
         : "memory");
 }
 
-// non-blocking phase test (mbarrier.test_wait): true once the phase with the given parity has completed
-__device__ __forceinline__ bool mbar_test(uint64_t* bar, uint32_t parity) {
-    uint32_t ok;
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "mbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t"
-        "}\n"
-        : "=r"(ok)
-        : "r"(smem_u32(bar)), "r"(parity)
-        : "memory");
-    return ok != 0;
-}
-
 // ------------------------------------------------------------------ TMA loads (tile mode)
-__device__ __forceinline__ void tma_load_2d(const CUtensorMap* map, uint64_t* bar, void* dst, int c0, int c1) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::"r"(
-            smem_u32(dst)),
-        "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
-        : "memory");
-}
 __device__ __forceinline__ void tma_load_4d(const CUtensorMap* map, uint64_t* bar, void* dst, int c0, int c1, int c2,
                                             int c3) {
     asm volatile(
@@ -76,169 +53,31 @@ __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* map) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(map)) : "memory");
 }
 
-// ------------------------------------------------------------------ TMEM
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)),
-                 "r"(ncols)
-                 : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void fence_before_sync() {
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void fence_after_sync() {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// make the completion of all prior tcgen05.mma of this thread arrive on an mbarrier
-__device__ __forceinline__ void mma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-                 : "memory");
-}
-
-// D[tmem] (+)= A[smem] * B[smem]^T, fp16/bf16 inputs, one thread issues
-__device__ __forceinline__ void mma_f16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                        uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}\n" ::"r"(tmem_d),
-        "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-
-// ------------------------------------------------------------------ CTA pairs (cta_group::2): two SMs of one TPC issue one
-// 256-row MMA; each CTA stages its own 128 rows of A and HALF of the B tile, so the shared-memory fill and operand-read
-// traffic per SM drops by ~30-50 % (the 1-SM kernel is shared-memory-bandwidth bound on this part).
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-    return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// shared::cluster address of `smem_addr` (a shared::cta address of this CTA) in the CTA with rank `rank`
-__device__ __forceinline__ uint32_t mapa_u32(uint32_t smem_addr, uint32_t rank) {
-    uint32_t r;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(smem_addr), "r"(rank));
-    return r;
-}
-// arrive on an mbarrier given by its shared::cluster address (possibly in the peer CTA)
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
-    asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-// TMA tile load issued by either CTA of a pair: data lands in THIS CTA's shared memory, the transaction bytes are
-// credited to the mbarrier at shared::cluster address `bar_cluster_addr` (the leader CTA's full barrier)
-__device__ __forceinline__ void tma_load_4d_pair(const CUtensorMap* map, uint32_t bar_cluster_addr, void* dst, int c0, int c1,
-                                                 int c2, int c3) {
-    asm volatile(
-        "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, "
-        "%6}], [%2];" ::"r"(smem_u32(dst)),
-        "l"(reinterpret_cast<uint64_t>(map)), "r"(bar_cluster_addr), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_alloc_pair(uint32_t* smem_dst, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)), "r"(ncols)
-                 : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish_pair() {
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_pair(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// D[tmem of both CTAs] (+)= A[256 rows: 128 per CTA] * B[N rows: N/2 per CTA]^T; issued by one thread of the leader CTA
-__device__ __forceinline__ void mma_f16_pair(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                             uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}\n" ::"r"(tmem_d),
-        "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// completion of all prior pair-MMAs arrives on the mbarrier at this shared-memory offset in BOTH CTAs (mask 0b11)
-__device__ __forceinline__ void mma_commit_pair(uint64_t* bar) {
-    asm volatile(
-        "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-            smem_u32(bar)),
-        "h"(static_cast<uint16_t>(3))
-        : "memory");
-}
-
-// 32 lanes x 32 columns of fp32: thread i of the warp receives row (lane base + i), 32 consecutive columns
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t* v) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-          "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-          "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-          "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-        : "r"(taddr)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// 256-bit global accesses (sm_100: LDG/STG.E.ENL2.256): one full 32-byte sector per thread per instruction.  Row-per-
-// thread epilogues write 64-byte runs; with 128-bit stores every sector is written twice as two partial 16-byte halves.
-__device__ __forceinline__ void st_global_256(void* ptr, const uint4& a, const uint4& b) {
-    asm volatile("st.global.v8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"l"(ptr), "r"(a.x), "r"(a.y), "r"(a.z),
-                 "r"(a.w), "r"(b.x), "r"(b.y), "r"(b.z), "r"(b.w)
-                 : "memory");
-}
-__device__ __forceinline__ void ld_global_256(const void* ptr, uint4& a, uint4& b) {
-    asm volatile("ld.global.nc.v8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-                 : "=r"(a.x), "=r"(a.y), "=r"(a.z), "=r"(a.w), "=r"(b.x), "=r"(b.y), "=r"(b.z), "=r"(b.w)
-                 : "l"(ptr));
-}
-
-// ------------------------------------------------------------------ descriptors
-// K-major operand tile, rows of 64 fp16 (128 B) with 128-byte swizzle: 8-row atoms of 1024 B.
-//   start address >> 4 | LBO (unused for swizzled K-major, 1) << 16 | SBO (1024 B >> 4) << 32 |
-//   version 1 << 46 | layout SWIZZLE_128B (2) << 61
+// ------------------------------------------------------------------ warpgroup MMA
+// K-major operand tile, rows of 64 fp16 (128 B) with 128-byte swizzle (the layout the TMA maps write): 8-row atoms of
+// 1024 B.  start address >> 4 | LBO (unused for swizzled K-major, 1) << 16 | SBO (1024 B >> 4) << 32 | SWIZZLE_128B << 62.
+// Tiles are 1024-byte aligned; a k-step of 16 elements inside the 128-byte row advances the start address by 32 bytes.
 __device__ __forceinline__ uint64_t make_desc_sw128(uint32_t smem_addr) {
     uint64_t d = 0;
     d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
     d |= static_cast<uint64_t>(1) << 16;
     d |= static_cast<uint64_t>(1024 >> 4) << 32;
-    d |= static_cast<uint64_t>(1) << 46;
-    d |= static_cast<uint64_t>(2) << 61;
+    d |= static_cast<uint64_t>(1) << 62;
     return d;
 }
-// low word of that descriptor; +2 per 32 bytes of start address (the high word is the constant DESC_SW128_HI)
-__device__ __forceinline__ uint32_t desc_lo_sw128(uint32_t smem_addr) { return ((smem_addr & 0x3FFFF) >> 4) | (1u << 16); }
-constexpr uint32_t DESC_SW128_HI = (1024u >> 4) | (1u << 14) | (2u << 29);
-// same MMA with the descriptors given by their low words: the single issuing thread spends ~3 instructions per MMA
-// on operands instead of rebuilding two 64-bit descriptors (matters when one thread feeds 12+ MMAs per key tile)
-__device__ __forceinline__ void mma_f16_lo(uint32_t tmem_d, uint32_t lo_a, uint32_t lo_b, uint32_t idesc,
-                                           uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        ".reg .b64 da, db;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "mov.b64 da, {%1, %5};\n\t"
-        "mov.b64 db, {%2, %5};\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %3, p;\n\t"
-        "}\n" ::"r"(tmem_d),
-        "r"(lo_a), "r"(lo_b), "r"(idesc), "r"(accumulate), "r"(DESC_SW128_HI)
-        : "memory");
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+    asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
+}
+// registers that a wgmma still in flight accumulates into must not be touched by other code: this pins them
+template <int R>
+__device__ __forceinline__ void reg_fence(float* d) {
+#pragma unroll
+    for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// kind::f16, fp16 A/B (format 0), fp32 accumulate (c_format 1), both K-major, dense
-__host__ __device__ constexpr uint32_t make_idesc_f16(int M, int N) {
-    return (1u << 4) | (static_cast<uint32_t>(N >> 3) << 17) | (static_cast<uint32_t>(M >> 4) << 24);
-}
+#include "rf_wgmma.inc"
 
 }  // namespace tc

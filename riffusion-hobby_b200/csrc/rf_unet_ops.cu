@@ -715,7 +715,7 @@ __global__ void k_slerp_apply(const __half* __restrict__ v0, const __half* __res
 
 inline unsigned grid_for(size_t n, int block) {
     size_t g = (n + block - 1) / block;
-    return static_cast<unsigned>(g > 148 * 16 ? 148 * 16 : (g ? g : 1));
+    return static_cast<unsigned>(g > 132 * 16 ? 132 * 16 : (g ? g : 1));
 }
 
 }  // namespace
@@ -747,7 +747,7 @@ extern "C" int rf_group_norm_cat_f16(const void* x, const void* x2, int C1, int 
     const int threads = PPI * C8;
     // slab: >= 32 pixels (the scratch is sized for HW/32 slabs); large images take longer slabs (still >= 4 waves)
     int slab = 32;
-    while (slab < 256 && static_cast<long>(B) * (HW / (2 * slab)) >= 4 * 148) slab *= 2;
+    while (slab < 256 && static_cast<long>(B) * (HW / (2 * slab)) >= 4 * 132) slab *= 2;
     const int nslabs = (HW + slab - 1) / slab;
     float* part = d_scratch + static_cast<size_t>(B) * groups * 2;     // [B][nslabs][G][2]
     const size_t smem = static_cast<size_t>(PPI) * (C / 2) * sizeof(float2);
@@ -868,7 +868,7 @@ static int launch_conv_in_blk(const void* x, const void* w, const void* bias, in
     const size_t smem = (static_cast<size_t>(64 * NCO2) * Cin * 9 + 8 * 18 * 8) * sizeof(float);
     RF_CUDA_TRY(cudaFuncSetAttribute(k_conv_in_blk<NCO2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
     const long ngroups = static_cast<long>(B) * H * (W / 4);
-    const unsigned grid = static_cast<unsigned>(std::min<long>((ngroups + 7) / 8, 2 * 148));
+    const unsigned grid = static_cast<unsigned>(std::min<long>((ngroups + 7) / 8, 2 * 132));
     k_conv_in_blk<NCO2><<<grid, 256, smem, st>>>(static_cast<const __half*>(x), static_cast<const __half*>(w),
                                                  static_cast<const __half*>(bias), B, Cin, H, W, static_cast<__half*>(y));
     RF_CUDA_LAUNCH_CHECK("k_conv_in_blk");
@@ -907,7 +907,7 @@ static int launch_conv_out_blk(const void* x, const void* w, const void* bias, i
     const size_t smem = static_cast<size_t>(9) * NSTEP * 256 * sizeof(float);
     RF_CUDA_TRY(cudaFuncSetAttribute(k_conv_out_blk<NSTEP>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
     const long ngroups = static_cast<long>(B) * H * (W / 4);
-    const unsigned grid = static_cast<unsigned>(std::min<long>((ngroups + 7) / 8, 2 * 148));
+    const unsigned grid = static_cast<unsigned>(std::min<long>((ngroups + 7) / 8, 2 * 132));
     k_conv_out_blk<NSTEP><<<grid, 256, smem, st>>>(static_cast<const __half*>(x), static_cast<const __half*>(w),
                                                    static_cast<const __half*>(bias), B, H, W, Cout, static_cast<__half*>(y));
     RF_CUDA_LAUNCH_CHECK("k_conv_out_blk");

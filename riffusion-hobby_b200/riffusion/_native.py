@@ -2,7 +2,7 @@
 
 PyTorch is only plumbing here: tensors own the device memory, `data_ptr()` and the current
 CUDA stream are handed to the library.  There is no CPU fallback — if the library is missing
-or no sm_100 GPU is present, calls raise.
+or no sm_90 GPU (H100) is present, calls raise.
 """
 from __future__ import annotations
 
@@ -151,7 +151,7 @@ def lib() -> C.CDLL:
             if not _LIB_PATH.exists():
                 raise NativeError(
                     f"{_LIB_PATH} not found: build it with `python riffusion-hobby_b200/build.py` "
-                    "(nvcc, sm_100a). There is no CPU fallback."
+                    "(nvcc, sm_90a). There is no CPU fallback."
                 )
             handle = C.CDLL(str(_LIB_PATH))
             for name, (res, args) in SIGNATURES.items():

@@ -9,7 +9,7 @@ the same names, flags and defaults:
     python -m riffusion.cli sample-clips-batch --audio-dir songs --output-dir clips
 
 Each command is a keyword-only function (callable from Python exactly like the reference's); `argh`, which the reference
-uses to turn those functions into sub-commands, is not installed on the B200 image, so `build_parser` derives an
+uses to turn those functions into sub-commands, is not installed on the GPU image, so `build_parser` derives an
 argparse sub-command per function from its signature instead.  Audio I/O goes through riffusion.util.audio_util
 (pydub when present, else the WAV-only stand-in).
 """

@@ -1,5 +1,5 @@
 """ClipTextB200 — the CLIP text encoder (openai/clip-vit-large-patch14 text tower: 12 layers, width 768, 12 heads, MLP 3072,
-quick_gelu, 77 positions, causal attention) on this library's tcgen05 GEMM / attention kernels (SURVEY §8(f)-3).
+quick_gelu, 77 positions, causal attention) on this library's wgmma GEMM / attention kernels (SURVEY §8(f)-3).
 
 Seam: `RiffusionPipeline.embed_text` / `embed_text_weighted` call `self.text_encoder(input_ids)[0]`
 (riffusion/riffusion_pipeline.py:177-206, external/prompt_weighting.py:194-234); the reference's object there is

@@ -1,7 +1,7 @@
 """Request / response schema of the inference API.
 
 Field names, order and defaults are those of the reference's riffusion/datatypes.py:10-73 (the Flask server fills them
-from request JSON with `dacite`; that package is not on the B200 image, so `from_dict` below does the same nested
+from request JSON with `dacite`; that package is not on the GPU image, so `from_dict` below does the same nested
 construction for the two input types, rejecting unknown keys like dacite's strict mode).
 """
 from __future__ import annotations

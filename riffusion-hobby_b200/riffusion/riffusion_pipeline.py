@@ -1,8 +1,8 @@
-"""RiffusionPipeline — B200-native drop-in for riffusion/riffusion_pipeline.py.
+"""RiffusionPipeline — H100-native drop-in for riffusion/riffusion_pipeline.py.
 
 Same public surface as the reference class (`load_checkpoint`, `riffuse`, `interpolate_img2img`, `embed_text`,
 `embed_text_weighted`, `device`, module-level `preprocess_image` / `preprocess_mask`) and the same control flow
-around the inner seams (`self.unet(...)`, `self.scheduler.*`, `self.vae.*`), but those seams are the tcgen05
+around the inner seams (`self.unet(...)`, `self.scheduler.*`, `self.vae.*`), but those seams are the wgmma
 implementations of this package (UNetB200, PNDMSchedulerB200, VaeB200) instead of diffusers modules.
 
 What is NOT here: diffusers (`DiffusionPipeline.from_pretrained`, hub download, traced-UNet download) — none of
@@ -34,7 +34,7 @@ VAE_SCALE = 0.18215
 
 
 class RiffusionPipeline:
-    """Prompt / seed interpolation on spectrogram images (img2img), running on one B200."""
+    """Prompt / seed interpolation on spectrogram images (img2img), running on one H100."""
 
     def __init__(self, vae: VaeB200, unet: UNetB200, scheduler: T.Optional[PNDMSchedulerB200] = None,
                  text_encoder=None, tokenizer=None, device: str = "cuda"):
@@ -64,11 +64,11 @@ class RiffusionPipeline:
                         low_cpu_mem_usage: bool = False, cache_dir: T.Optional[str] = None) -> "RiffusionPipeline":
         """Load a diffusers-layout checkpoint directory (`unet/diffusion_pytorch_model.{safetensors,bin}`,
         `vae/...`, optional `text_encoder/`, `tokenizer/`).  Signature kept from riffusion_pipeline.py:63-125;
-        `use_traced_unet` / `channels_last` are accepted and ignored (the tcgen05 UNet already is the fast path,
+        `use_traced_unet` / `channels_last` are accepted and ignored (the wgmma UNet already is the fast path,
         activations are always channels-last)."""
         device = torch_util.check_device(device)
         if dtype != torch.float16:
-            raise ValueError("the B200-native pipeline computes in fp16 (the reference forces fp32 only on CPU/MPS)")
+            raise ValueError("the H100-native pipeline computes in fp16 (the reference forces fp32 only on CPU/MPS)")
         root = Path(checkpoint)
         if not root.is_dir():
             raise FileNotFoundError(

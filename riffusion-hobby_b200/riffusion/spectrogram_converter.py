@@ -1,4 +1,4 @@
-"""SpectrogramConverter — B200-native drop-in for riffusion/spectrogram_converter.py.
+"""SpectrogramConverter — H100-native drop-in for riffusion/spectrogram_converter.py.
 
 Same constructor, public attributes (`p`, `device`, `spectrogram_func`,
 `inverse_spectrogram_func`, `mel_scaler`, `inverse_mel_scaler`) and methods as the reference
@@ -217,7 +217,7 @@ class GriffinLim(_Transform):
 
 
 class SpectrogramConverter:
-    """Convert between audio segments and mel-amplitude spectrogram tensors on a B200.
+    """Convert between audio segments and mel-amplitude spectrogram tensors on an H100.
 
     See the reference class docstring (spectrogram_converter.py:12-32) for the semantics; a
     "spectrogram" here is (channels, n_mels, frames) of mel amplitudes.
@@ -234,7 +234,7 @@ class SpectrogramConverter:
             self.device = "cpu"
         if not str(self.device).lower().startswith("cuda"):
             raise RuntimeError(
-                f"SpectrogramConverter(device={device!r}): the B200-native build runs the audio path "
+                f"SpectrogramConverter(device={device!r}): the H100-native build runs the audio path "
                 "in CUDA kernels only; there is no CPU implementation"
             )
         # validates the geometry now (raises NotImplementedError for unsupported sizes)

@@ -1,7 +1,7 @@
 """Thin tensor wrappers over the tensor-core C-ABI entry points (rf_gemm_f16, rf_conv2d_f16, ...).
 
 Activations are fp16, NHWC for images and (rows, channels) for token matrices.  These helpers only
-marshal pointers/strides; every FLOP runs in the tcgen05 kernels of librf_b200.so.
+marshal pointers/strides; every FLOP runs in the wgmma kernels of librf_b200.so.
 """
 from __future__ import annotations
 
@@ -331,7 +331,7 @@ def conv1x1_small(x_nchw: torch.Tensor, w: torch.Tensor, bias: torch.Tensor, in_
 
 
 def attention(q: torch.Tensor, k: torch.Tensor, vt: torch.Tensor, heads: int, nk: int, causal: bool = False) -> torch.Tensor:
-    """q: (B, Nq, C), k: (B, >=nk, C), vt: (B, C, pitch>=nk) fp16 contiguous -> (B, Nq, C); fused tcgen05 kernel.
+    """q: (B, Nq, C), k: (B, >=nk, C), vt: (B, C, pitch>=nk) fp16 contiguous -> (B, Nq, C); fused wgmma kernel.
     causal: key j is visible to query i iff j <= i (text encoder; nk <= 128)."""
     _f16(q, "q"), _f16(k, "k"), _f16(vt, "vt")
     B, Nq, C = q.shape

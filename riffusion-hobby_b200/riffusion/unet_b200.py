@@ -1,4 +1,4 @@
-"""UNetB200 — the SD-1.5 UNet2DConditionModel forward on tcgen05 kernels.
+"""UNetB200 — the SD-1.5 UNet2DConditionModel forward on wgmma kernels.
 
 Drop-in at the reference's own UNet seam: `RiffusionPipeline` calls
 `self.unet(latent_model_input, t, encoder_hidden_states=...)` and reads `.sample`
@@ -11,7 +11,7 @@ UNet2DConditionModel, see oracle/unet_oracle.py) and are repacked once: 3x3 conv
 [Cout][ky][kx][Cin] (K-major for the implicit-GEMM TMA stream), everything fp16.  Activations are NHWC
 fp16 end to end; the only NCHW tensors are the 4-channel latents at the two edge convolutions.
 
-Every FLOP runs in librf_b200.so: convs and linears in the tcgen05/TMEM kernel (rf_conv2d_f16 /
+Every FLOP runs in librf_b200.so: convs and linears in the wgmma kernel (rf_conv2d_f16 /
 rf_gemm_f16), norms / GEGLU / softmax in the memory-bound kernels of rf_unet_ops.cu.  No torch.nn,
 cuDNN or cuBLAS call is made on this path; torch only allocates tensors and provides the stream.
 """

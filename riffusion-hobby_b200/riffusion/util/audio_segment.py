@@ -1,6 +1,6 @@
 """Minimal numpy-backed stand-in for pydub.AudioSegment.
 
-pydub (and ffmpeg) are not installed in the B200 image, but the reference API passes
+pydub (and ffmpeg) are not installed in the GPU image, but the reference API passes
 `pydub.AudioSegment` objects across `SpectrogramConverter.spectrogram_from_audio` /
 `audio_from_spectrogram` (spectrogram_converter.py:101-163).  When pydub is importable it is
 used; otherwise this class provides the subset of its surface the converter, the image

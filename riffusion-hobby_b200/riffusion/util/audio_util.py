@@ -1,7 +1,7 @@
 """Audio helpers (reference: riffusion/util/audio_util.py).
 
 pydub is used when it is installed; otherwise the numpy AudioSegment stand-in from
-`audio_segment.py` is (pydub/ffmpeg are absent from the B200 image).
+`audio_segment.py` is (pydub/ffmpeg are absent from the GPU image).
 """
 from __future__ import annotations
 

@@ -19,7 +19,7 @@ def check_device(device: str, backup: str = "cpu") -> str:
     wanted = device.lower()
     if wanted.startswith("cuda") and not torch.cuda.is_available():
         raise RuntimeError(
-            f"{device} is not available and the B200-native riffusion build has no CPU fallback "
+            f"{device} is not available and the H100-native riffusion build has no CPU fallback "
             f"(the reference would have warned and used {backup})"
         )
     if wanted.startswith("mps"):

@@ -1,4 +1,4 @@
-"""VaeB200 — AutoencoderKL decode / encode-moments on the same tcgen05 conv/GEMM kernels as the UNet.
+"""VaeB200 — AutoencoderKL decode / encode-moments on the same wgmma conv/GEMM kernels as the UNet.
 
 Seams it sits behind: `self.vae.decode(latents).sample` (riffusion/riffusion_pipeline.py:427-428) and
 `self.vae.encode(image).latent_dist.sample(generator=...)` (:255-264).  Weights: diffusers-format AutoencoderKL

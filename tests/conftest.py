@@ -15,7 +15,7 @@ GOLDEN = ROOT / "tests" / "golden"
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
     # the torch oracles are "fp32" checkers: keep cuDNN / cuBLAS from silently using TF32 (10-bit mantissa) for them
     import torch
 

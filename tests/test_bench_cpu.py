@@ -1,5 +1,5 @@
 """bench.py contract checks that need no GPU: the reference arm (`--impl reference`) must print ONE JSON line with the
-B200 arm's metric / unit / config for the same workload, so that the driver can form the ratio of the two arms."""
+GPU arm's metric / unit / config for the same workload, so that the two arms' results form a ratio."""
 import json
 import subprocess
 import sys
@@ -23,7 +23,7 @@ def test_reference_arm_clip_workload_line():
 
     d = _run("--evals", "50", "--clips", "32")
     assert d["impl"] == "reference" and d["metric"] == "clips/sec" and d["unit"] == "clips/s" and d["higher_is_better"]
-    assert d["config"] == bench.clip_config(50, 50, 32)          # identical to the B200 arm's config for these flags
+    assert d["config"] == bench.clip_config(50, 50, 32)          # identical to the GPU arm's config for these flags
     assert d["value"] > 0 and d["cpu_baseline"]["value"] == d["value"] and d["cpu_baseline"]["kind"] in ("port", "reference")
     assert d["e2e"] == {"value": d["value"], "unit": "clips/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0}
     assert d["gpu_launches"] == 0 and "sample" in d["cpu_baseline"] and d["cpu_baseline"]["cores"] >= 1

@@ -38,7 +38,7 @@ def test_audio_to_image_then_image_to_audio(native_lib, golden, tmp_path, stereo
 
 
 def test_server_compute_request_on_gpu(native_lib, tmp_path):
-    """riffusion/server.py:116-183 end to end on the GPU: riffuse (reduced-width UNet + full VAE + B200 CLIP encoder) ->
+    """riffusion/server.py:116-183 end to end on the GPU: riffuse (reduced-width UNet + full VAE + library's CLIP encoder) ->
     SpectrogramImageConverter.audio_from_spectrogram_image -> JSON with a base64 JPEG and base64 audio of 5.11 s"""
     import base64
     import io

@@ -1,4 +1,4 @@
-"""(f)-3: ClipTextB200 (the CLIP text encoder on the tcgen05 GEMM / causal-attention kernels) against the reference's own
+"""(f)-3: ClipTextB200 (the CLIP text encoder on the wgmma GEMM / causal-attention kernels) against the reference's own
 dependency for this module — `transformers.CLIPTextModel` (what diffusers loads as `pipe.text_encoder`,
 riffusion/riffusion_pipeline.py:92-102,177-191) — built offline with the CLIP-L/14 text configuration and random-init
 weights; both sides hold the same fp16-representable parameters.  The oracle here is PINNED: it is the real library."""
@@ -57,7 +57,7 @@ def test_clip_text_encoder_matches_transformers(clip_pair):
 
 @torch.no_grad()
 def test_pipeline_embeds_text_through_b200_encoder(clip_pair):
-    """embed_text / embed_text_weighted (riffusion_pipeline.py:177-206) with the B200 encoder behind the tokenizer seam"""
+    """embed_text / embed_text_weighted (riffusion_pipeline.py:177-206) with the library's encoder behind the tokenizer seam"""
     import sys
     from pathlib import Path
 

@@ -22,7 +22,7 @@ def test_header_symbols_exported(native_lib):
     assert declared == set(_native.SIGNATURES), declared ^ set(_native.SIGNATURES)
     for name in declared:
         assert hasattr(native_lib, name)
-    assert b"sm_100a" in native_lib.rf_version()
+    assert b"sm_90a" in native_lib.rf_version()
 
 
 def test_no_cpu_fallback_without_gpu(native_lib):

@@ -1,4 +1,4 @@
-"""GPU numerics of the tcgen05 GEMM / implicit-GEMM convolution against plain PyTorch fp32 references
+"""GPU numerics of the wgmma GEMM / implicit-GEMM convolution against plain PyTorch fp32 references
 of the same op (fp16-rounded inputs, fp32 math).  Tolerance: fp16 output rounding (2^-11 relative) plus
 fp32 accumulation-order noise: |err| <= 2e-3 * max|ref| everywhere."""
 import pytest
@@ -110,7 +110,7 @@ def test_conv_matches_torch(native_lib, B, H, W, C1, C2, Cout, k, stride):
                                              (3, 8, 64, 64, 160), (2, 8, 4096, 77, 40), (1, 8, 1024, 77, 80),
                                              (2, 8, 256, 77, 160), (1, 4, 200, 300, 16), (1, 2, 128, 129, 64)])
 def test_fused_attention_matches_torch(native_lib, B, heads, Nq, Nk, d):
-    """fused QK^T -> softmax -> PV (tcgen05) vs fp32 torch attention on the same fp16 inputs;
+    """fused QK^T -> softmax -> PV (wgmma) vs fp32 torch attention on the same fp16 inputs;
     UNet self-/cross-attention shapes plus ragged sizes (query / key tails, single and odd tile counts)"""
     from riffusion import tc_ops
 
@@ -133,8 +133,8 @@ def test_fused_attention_matches_torch(native_lib, B, heads, Nq, Nk, d):
 
 @pytest.mark.parametrize("Nk,d", [(1024, 40), (700, 40), (512, 80), (384, 64), (300, 96)])
 def test_fused_attention_growing_scores(native_lib, Nk, d):
-    """single-pass kernel: the keys are ordered so that the row maximum keeps growing along the key axis (forces the
-    TMEM rescale of the running accumulators several times per row) with peaked softmax rows (large logits)"""
+    """online softmax: the keys are ordered so that the row maximum keeps growing along the key axis (forces the
+    rescale of the running accumulators on every key tile) with peaked softmax rows (large logits)"""
     from riffusion import tc_ops
 
     torch.manual_seed(Nk + d)
@@ -158,31 +158,33 @@ def test_fused_attention_growing_scores(native_lib, Nk, d):
     assert float((got.float() - ref).norm() / ref.norm()) < 3e-3
 
 
-# ----------------------------------------------------------------------------------------------- CTA-pair kernel
-def _pair_env(bn):
+# ----------------------------------------------------------------------------------------------- tile widths
+def _tile_env(bn, bres="1"):
     import os
 
-    os.environ.pop("RF_GEMM_PAIR", None)
     if bn is None:
         os.environ.pop("RF_GEMM_BN", None)
     else:
         os.environ["RF_GEMM_BN"] = str(bn)
+    if bres == "0":
+        os.environ["RF_GEMM_BRES"] = "0"
+    else:
+        os.environ.pop("RF_GEMM_BRES", None)
 
 
-@pytest.mark.parametrize("bn", [None, 320, 256, 160, 128])
-def test_pair_kernel_gemm_matches_torch_and_single_cta(native_lib, bn):
-    """problems large enough for the cta_group::2 kernel (256 x BN tiles on CTA pairs), every tile width, ragged M
-    (odd number of 128-row blocks: the second CTA of the last pair is fully out of bounds), bias / SiLU / residual /
-    GEGLU epilogues, batched operands; results also compared with the 1-SM kernel (RF_GEMM_PAIR=0)"""
-    import os
-
+@pytest.mark.parametrize("bres", ["1", "0"])
+@pytest.mark.parametrize("bn", [None, 64, 128, 160])
+def test_large_gemm_matches_torch_every_tile_width(native_lib, bn, bres):
+    """problems of many waves with every output-tile width (RF_GEMM_BN) and with the B-stationary mode on and off, ragged M
+    (a partial last 128-row block), bias / SiLU / residual / GEGLU epilogues, batched operands; results also compared with
+    the default tile choice"""
     import torch.nn.functional as F
 
     from riffusion import tc_ops as ops
 
     try:
         for (M, N, K) in ((128 * 297 - 58, 320, 320), (40000, 1280, 640), (36000, 640, 320), (38000, 256, 192)):
-            if (bn == 160 and N % 160) or (bn == 320 and N % 320):
+            if bn == 160 and N % 160:
                 continue
             torch.manual_seed(M + N)
             a = (torch.randn(M, K, device="cuda") * 0.5).half()
@@ -190,20 +192,19 @@ def test_pair_kernel_gemm_matches_torch_and_single_cta(native_lib, bn):
             bias = torch.randn(N, device="cuda").half()
             res = torch.randn(M, N, device="cuda").half()
             ref = a.float() @ b.float().t()
-            _pair_env(bn)
+            _tile_env(bn, bres)
             g1 = ops.gemm(a, b).reshape(M, N)
             g2 = ops.gemm(a, b, bias=bias, residual=res, alpha=0.5).reshape(M, N)
             g3 = ops.gemm(a, b, bias=bias, act=ops.ACT_SILU).reshape(M, N)
             _close(g1, ref)
             _close(g2, 0.5 * ref + bias.float() + res.float())
             _close(g3, F.silu(ref + bias.float()))
-            os.environ["RF_GEMM_PAIR"] = "0"
+            _tile_env(None)
             s1 = ops.gemm(a, b).reshape(M, N)
-            # same K order inside a tile and fp32 accumulation in TMEM: the two kernels agree (to the last bit, if the
-            # 256-row instruction accumulates like the 128-row one; at most isolated fp16 rounding flips otherwise)
+            # same K order and fp32 accumulation for every tile width: at most isolated fp16 rounding flips
             assert float((g1 != s1).float().mean()) < 1e-3 and float((g1.float() - s1.float()).abs().max()) <= 2e-3 * float(ref.abs().max()), (M, N, K)
         # GEGLU epilogue (N = 8C interleaved) and a batched V^T-style product with 3 row blocks per batch entry
-        _pair_env(bn)
+        _tile_env(bn, bres)
         M, C = 33000, 320
         x = torch.randn(M, C, device="cuda").half()
         w = (torch.randn(8 * C, C, device="cuda") / C ** 0.5).half()
@@ -218,7 +219,7 @@ def test_pair_kernel_gemm_matches_torch_and_single_cta(native_lib, bn):
         ops.gemm(wv, xt.unsqueeze(1), out=vt)
         _close(vt.reshape(Bt, 320, T), torch.einsum("ck,btk->bct", wv.float(), xt.float()))
     finally:
-        _pair_env(None)
+        _tile_env(None)
 
 
 @pytest.mark.parametrize("B,H,W,C1,C2,Cout,k,stride", [
@@ -226,11 +227,10 @@ def test_pair_kernel_gemm_matches_torch_and_single_cta(native_lib, bn):
     (16, 64, 64, 320, 0, 320, 3, 2), (13, 48, 48, 128, 0, 256, 3, 1), (24, 32, 32, 960, 0, 640, 1, 1),
     (3, 256, 256, 128, 0, 128, 3, 1),
 ])
-def test_pair_kernel_conv_matches_torch(native_lib, B, H, W, C1, C2, Cout, k, stride):
-    """implicit-GEMM convolution on CTA pairs: each CTA of a pair gathers its own 128 output pixels (TMA im2col boxes),
-    stride 2, channel concat through the second tensor map, per-image bias, residual; vs torch and vs the 1-SM kernel"""
-    import os
-
+def test_large_conv_matches_torch_every_tile_width(native_lib, B, H, W, C1, C2, Cout, k, stride):
+    """implicit-GEMM convolution at batch sizes of many waves: each CTA gathers its 128 output pixels (TMA im2col boxes),
+    stride 2, channel concat through the second tensor map, per-image bias, residual; vs torch with the default tile
+    width, and the default vs the 128- and 64-column tiles"""
     from riffusion import tc_ops
 
     torch.manual_seed(H + C1 + Cout + k)
@@ -245,17 +245,18 @@ def test_pair_kernel_conv_matches_torch(native_lib, B, H, W, C1, C2, Cout, k, st
     ref = (ref + temb.float()[:, :, None, None]).permute(0, 2, 3, 1)
     wp = tc_ops.pack_conv_weight(w)
     try:
-        _pair_env(None)
+        _tile_env(None)
         got = tc_ops.conv2d(x, wp, x2=x2, bias=bias, bias_per_image=temb, stride=stride)
         _close(got, ref)
         res = torch.randn_like(got)
         got2 = tc_ops.conv2d(x, wp, x2=x2, bias=bias, residual=res, stride=stride)
         _close(got2, ref - temb.float()[:, None, None, :] + res.float())
-        os.environ["RF_GEMM_PAIR"] = "0"
-        single = tc_ops.conv2d(x, wp, x2=x2, bias=bias, bias_per_image=temb, stride=stride)
-        assert float((got != single).float().mean()) < 1e-3
+        for bn in (128, 64):
+            _tile_env(bn)
+            other = tc_ops.conv2d(x, wp, x2=x2, bias=bias, bias_per_image=temb, stride=stride)
+            assert float((got != other).float().mean()) < 1e-3, bn
     finally:
-        _pair_env(None)
+        _tile_env(None)
 
 
 @pytest.mark.parametrize("B,H,W,Cin,Cout", [(2, 16, 16, 1280, 1280), (2, 32, 32, 640, 640), (1, 8, 8, 128, 64),
