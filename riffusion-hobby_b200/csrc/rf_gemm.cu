@@ -81,8 +81,9 @@ __device__ __forceinline__ float apply_act(float v, int act) {
 }
 
 // exact-erf GELU  g * Phi(g),  Phi(g) = 0.5 erfc(-g / sqrt 2), branch-free with ONE MUFU op:
-//   0.5 erfc(t) = 2^q(t) on t = |g| / sqrt 2 in [0, 4] (degree-7 fit of -log2 erfc(t) - 1; erfc(4) = 1.5e-8, clamped
-//   beyond), Phi = g < 0 ? h : 1 - h.  |error| <= 7e-7 absolute, <= 4.2e-6 relative (fp32 Horner), i.e. 1 % of an fp16 ulp —
+//   0.5 erfc(t) = 2^q(t) on t = |g| / sqrt 2 in [0, 4) (degree-7 fit of -log2 erfc(t) - 1; erfc(4) = 1.5e-8, and
+//   h = 0 beyond: a clamped h = 7.7e-9 times a large negative g would give g * h, -5e-4 at g = -65504 instead of -0),
+//   Phi = g < 0 ? h : 1 - h.  |error| <= 7e-7 absolute, <= 4.2e-6 relative (fp32 Horner), i.e. 1 % of an fp16 ulp —
 //   same function as erff's GELU (diffusers GEGLU uses the exact form), not the tanh approximation.  erff() costs ~35
 //   instructions per element on two divergent paths.
 __device__ __forceinline__ float gelu_erf_fast(float g) {
@@ -97,7 +98,7 @@ __device__ __forceinline__ float gelu_erf_fast(float g) {
     q = fmaf(q, t, -0.9999938f);
     float h;
     asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(h) : "f"(q));
-    return g * (g < 0.f ? h : 1.f - h);
+    return g * (g < 0.f ? (t < 4.0f ? h : 0.f) : 1.f - h);
 }
 
 __device__ __forceinline__ void named_bar_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }

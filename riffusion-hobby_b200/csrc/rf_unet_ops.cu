@@ -35,13 +35,22 @@ __device__ __forceinline__ float silu(float v) { return v / (1.f + __expf(-v)); 
 //         repeated runs are bit-identical).
 // pass 2 (inside the apply kernel): the slab partials are added in a fixed order -> (mean, rstd) per group.
 // pass 3: y = (x - mean) * rstd * gamma + beta, optional SiLU.
+// Two pairs of sums are kept: the plain sum x and sum x^2, and sums shifted by a per-(image, group) pivot K, the mean of
+// the group's channels at pixel 0: sum (x - K) and sum (x - K)^2.  E[x^2] - mean^2 cancels in fp32 when |mean| >> std
+// (offset 256, std 1: rstd off by 1e-2); it loses about log2(E[x^2] / var) bits.  Up to E[x^2] = 8 var (3 bits, rstd
+// within about 2^-20) the plain form is used, with exactly the arithmetic it always had, so results on well-scaled
+// activations are unchanged bit for bit; beyond, E[(x-K)^2] - (mean-K)^2, whose K lies within about std / sqrt(C/G) of
+// the mean.
 // Vectorised pass 1 (C % 8 == 0, C <= 2560): blockDim = PPI * C/8 threads; a thread owns 8 fixed channels (one 16-byte
 // load per pixel) and walks every PPI-th pixel of the slab, four loads in flight.  Same deterministic two-level sum.
 // Two-source form (x2 != nullptr): the input is the channel concatenation [x | x2] (C1 + (C - C1) channels,
 // torch.cat([x, skip], dim=1) of the up blocks) read in place — a thread's 8 channels come from one of the two tensors.
+// The pivots are computed by every CTA of pass 1 (pixel 0 staged in shared memory, each group summed in channel order)
+// and stored by the slab-0 CTA for the apply kernel, which adds them back to the mean.
 __global__ void k_gn_partial_v(const __half* __restrict__ x, const __half* __restrict__ x2, int C1, int HW, int C, int G,
-                               int slab, int nslabs, float* __restrict__ part /*[B][nslabs][G][2]*/) {
-    extern __shared__ float2 shp[];  // [PPI][C/2]
+                               int slab, int nslabs, float* __restrict__ part /*[B][nslabs][G][2]*/,
+                               float* __restrict__ part_shift /*[B][nslabs][G][2]*/, float* __restrict__ pivots /*[B][G]*/) {
+    extern __shared__ float4 shp[];  // [PPI][C/2]
     rf_pdl_trigger();      // PDL (rf_common.h)
     rf_pdl_wait();
     const int b = blockIdx.y;
@@ -52,7 +61,34 @@ __global__ void k_gn_partial_v(const __half* __restrict__ x, const __half* __res
     const int C8 = (second ? C - C1 : C1) >> 3;              // row pitch of the source tensor in 16-byte units
     const uint4* xb = reinterpret_cast<const uint4*>((second ? x2 : x) + static_cast<size_t>(b) * HW * (C8 * 8)) +
                       (second ? c8 - (C1 >> 3) : c8);
-    float s[4] = {0.f, 0.f, 0.f, 0.f}, ss[4] = {0.f, 0.f, 0.f, 0.f};
+    // the 8 channels may straddle two groups; a channel pair never does (C / G is even): one pivot per pair
+    const int cpg = C / G;
+    __shared__ float piv_s[64];            // G <= 64
+    {
+        float* row0 = reinterpret_cast<float*>(shp);      // pixel 0 of the image, C floats (shp holds PPI * C)
+        if (pp == 0) {
+            const uint4 v = xb[0];
+            const __half2* h = reinterpret_cast<const __half2*>(&v);
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+                const float2 f = __half22float2(h[j]);
+                row0[c8 * 8 + 2 * j] = f.x;
+                row0[c8 * 8 + 2 * j + 1] = f.y;
+            }
+        }
+        __syncthreads();
+        for (int g = threadIdx.x; g < G; g += blockDim.x) {
+            float a = 0.f;
+            for (int c = g * cpg; c < (g + 1) * cpg; ++c) a += row0[c];
+            piv_s[g] = __fdiv_rn(a, static_cast<float>(cpg));
+            if (blockIdx.x == 0) pivots[b * G + g] = piv_s[g];
+        }
+        __syncthreads();
+    }
+    float piv[4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) piv[j] = piv_s[(c8 * 8 + 2 * j) / cpg];
+    float s[4] = {0.f, 0.f, 0.f, 0.f}, ss[4] = {0.f, 0.f, 0.f, 0.f}, sd[4] = {0.f, 0.f, 0.f, 0.f}, ssd[4] = {0.f, 0.f, 0.f, 0.f};
     auto acc = [&](const uint4& v) {
         const __half2* h = reinterpret_cast<const __half2*>(&v);
 #pragma unroll
@@ -60,6 +96,9 @@ __global__ void k_gn_partial_v(const __half* __restrict__ x, const __half* __res
             const float2 f = __half22float2(h[j]);
             s[j] += f.x + f.y;
             ss[j] = fmaf(f.x, f.x, fmaf(f.y, f.y, ss[j]));
+            const float dx = f.x - piv[j], dy = f.y - piv[j];
+            sd[j] += dx + dy;
+            ssd[j] = fmaf(dx, dx, fmaf(dy, dy, ssd[j]));
         }
     };
     int p = p0 + pp;
@@ -70,20 +109,24 @@ __global__ void k_gn_partial_v(const __half* __restrict__ x, const __half* __res
     }
     for (; p < p1; p += PPI) acc(xb[static_cast<size_t>(p) * C8]);
 #pragma unroll
-    for (int j = 0; j < 4; ++j) shp[pp * C2 + c8 * 4 + j] = make_float2(s[j], ss[j]);
+    for (int j = 0; j < 4; ++j) shp[pp * C2 + c8 * 4 + j] = make_float4(s[j], ss[j], sd[j], ssd[j]);
     __syncthreads();
     const int cpg2 = (C / G) >> 1;
     for (int g = threadIdx.x; g < G; g += blockDim.x) {
-        float a = 0.f, q = 0.f;
+        float a = 0.f, q = 0.f, ad = 0.f, qd = 0.f;
         for (int w = 0; w < PPI; ++w)
             for (int k = 0; k < cpg2; ++k) {
-                const float2 v = shp[w * C2 + g * cpg2 + k];
+                const float4 v = shp[w * C2 + g * cpg2 + k];
                 a += v.x;
                 q += v.y;
+                ad += v.z;
+                qd += v.w;
             }
-        float* o = part + ((static_cast<size_t>(b) * nslabs + blockIdx.x) * G + g) * 2;
-        o[0] = a;
-        o[1] = q;
+        const size_t o = ((static_cast<size_t>(b) * nslabs + blockIdx.x) * G + g) * 2;
+        part[o] = a;
+        part[o + 1] = q;
+        part_shift[o] = ad;
+        part_shift[o + 1] = qd;
     }
 }
 
@@ -106,42 +149,67 @@ __device__ __forceinline__ float silu_exp(float v) {
 // Vectorised pass 3, same thread -> channel mapping: the affine form y = x * sc + sh (sc = rstd * gamma,
 // sh = beta - mean * sc) of the thread's 8 channels lives in registers for the whole slab.
 __global__ void k_gn_apply_v(const __half* __restrict__ x, const __half* __restrict__ x2, int C1,
-                             const float* __restrict__ part, int nslabs, float inv_n,
+                             const float* __restrict__ part, const float* __restrict__ part_shift,
+                             const float* __restrict__ pivots, int nslabs, float inv_n,
                              float eps, const __half* __restrict__ gamma, const __half* __restrict__ beta, int HW, int C,
                              int G, int act, int slab, __half* __restrict__ y) {
     // pass 2 folded in: every CTA reduces the slab partials of its image to (mean, rstd) per group — a few KB from L2, in a
-    // fixed order (P strided sub-sums per group, then added in index order), instead of a separate launch
+    // fixed order (P strided sub-sums per group, then added in index order), instead of a separate launch.  The shifted
+    // partials are only read when a group of this image needs them.
     __shared__ float st[64 * 2];              // [G][2] mean, rstd   (G <= 64)
     rf_pdl_trigger();      // PDL (rf_common.h)
     rf_pdl_wait();
-    __shared__ float sub[64 * 8 * 2];
+    __shared__ float2 sub[64 * 8];
+    __shared__ int shifted[64], any_shifted;
     const int b = blockIdx.y;
     {
         const int P = min(8, static_cast<int>(blockDim.x) / G);
         const int t = threadIdx.x;
-        if (t < G * P) {
-            const int g = t / P, pi = t - g * P;
-            float s = 0.f, ss = 0.f;
-            for (int i = pi; i < nslabs; i += P) {
-                const float* o = part + ((static_cast<size_t>(b) * nslabs + i) * G + g) * 2;
-                s += o[0];
-                ss += o[1];
+        auto slab_sums = [&](const float* src) {       // sub[g][pi] = sum over slabs pi, pi + P, ... of src
+            if (t < G * P) {
+                const int g = t / P, pi = t - g * P;
+                float a = 0.f, q = 0.f;
+                for (int i = pi; i < nslabs; i += P) {
+                    const float* o = src + ((static_cast<size_t>(b) * nslabs + i) * G + g) * 2;
+                    a += o[0];
+                    q += o[1];
+                }
+                sub[g * 8 + pi] = make_float2(a, q);
             }
-            sub[(g * 8 + pi) * 2] = s;
-            sub[(g * 8 + pi) * 2 + 1] = ss;
-        }
+        };
+        if (t == 0) any_shifted = 0;
+        slab_sums(part);
         __syncthreads();
+        float var = 0.f;
         if (t < G) {
             float s = 0.f, ss = 0.f;
             for (int pi = 0; pi < P; ++pi) {
-                s += sub[(t * 8 + pi) * 2];
-                ss += sub[(t * 8 + pi) * 2 + 1];
+                s += sub[t * 8 + pi].x;
+                ss += sub[t * 8 + pi].y;
             }
-            const float mean = s * inv_n;
-            const float var = fmaxf(ss * inv_n - mean * mean, 0.f);
+            // plain form, rounded explicitly as it always was: mean = s / n, var = fma(ss, 1/n, -mean^2)
+            const float mean = __fmul_rn(s, inv_n);
+            var = fmaxf(__fmaf_rn(ss, inv_n, -__fmul_rn(mean, mean)), 0.f);
             st[2 * t] = mean;
-            st[2 * t + 1] = rsqrtf(var + eps);
+            shifted[t] = __fmul_rn(mean, mean) > 7.f * var;       // E[x^2] > 8 var: take the shifted sums
+            if (shifted[t]) any_shifted = 1;
         }
+        __syncthreads();
+        if (any_shifted) {                    // block-uniform
+            slab_sums(part_shift);
+            __syncthreads();
+            if (t < G && shifted[t]) {
+                float sd = 0.f, ssd = 0.f;
+                for (int pi = 0; pi < P; ++pi) {
+                    sd += sub[t * 8 + pi].x;
+                    ssd += sub[t * 8 + pi].y;
+                }
+                const float dmean = sd * inv_n;           // mean - pivot
+                var = fmaxf(ssd * inv_n - dmean * dmean, 0.f);
+                st[2 * t] = pivots[b * G + t] + dmean;
+            }
+        }
+        if (t < G) st[2 * t + 1] = rsqrtf(var + eps);
         __syncthreads();
     }
     const int C8 = C >> 3;
@@ -203,16 +271,27 @@ __global__ void k_layernorm(const __half* __restrict__ x, const __half* __restri
     const int lane = threadIdx.x & 31;
     if (row >= rows) return;
     const __half2* xr = reinterpret_cast<const __half2*>(x + static_cast<size_t>(row) * C);
+    // plain form E[x^2] - mean^2 (explicit roundings, as it always computed); it cancels in fp32 when |mean| >> std, so
+    // beyond E[x^2] = 8 var (3 bits lost) a second pass computes sum (x - mean)^2
     float s = 0.f, ss = 0.f;
     for (int i = lane; i < C / 2; i += 32) {
         const float2 v = __half22float2(xr[i]);
         s += v.x + v.y;
-        ss += v.x * v.x + v.y * v.y;
+        ss = __fadd_rn(ss, __fmaf_rn(v.x, v.x, __fmul_rn(v.y, v.y)));
     }
     s = warp_sum(s);
     ss = warp_sum(ss);
-    const float mean = s / C;
-    const float rstd = rsqrtf(fmaxf(ss / C - mean * mean, 0.f) + eps);
+    const float mean = __fdiv_rn(s, static_cast<float>(C));
+    float var = fmaxf(__fmaf_rn(-mean, mean, __fdiv_rn(ss, static_cast<float>(C))), 0.f);
+    if (__fmul_rn(mean, mean) > 7.f * var) {
+        float sd = 0.f;
+        for (int i = lane; i < C / 2; i += 32) {
+            const float2 v = __half22float2(xr[i]);
+            sd = fmaf(v.x - mean, v.x - mean, fmaf(v.y - mean, v.y - mean, sd));
+        }
+        var = warp_sum(sd) / C;
+    }
+    const float rstd = rsqrtf(var + eps);
     __half2* yr = reinterpret_cast<__half2*>(y + static_cast<size_t>(row) * C);
     const __half2* g2 = reinterpret_cast<const __half2*>(gamma);
     const __half2* b2 = reinterpret_cast<const __half2*>(beta);
@@ -249,7 +328,7 @@ __global__ void __launch_bounds__(256) k_layernorm_v(const __half* __restrict__ 
         for (int j = 0; j < 4; ++j) {
             const float2 f = __half22float2(h[j]);
             s += f.x + f.y;
-            ss += f.x * f.x + f.y * f.y;
+            ss = __fadd_rn(ss, __fmaf_rn(f.x, f.x, __fmul_rn(f.y, f.y)));
         }
     }
 #pragma unroll
@@ -257,8 +336,29 @@ __global__ void __launch_bounds__(256) k_layernorm_v(const __half* __restrict__ 
         s += __shfl_xor_sync(0xffffffffu, s, o);
         ss += __shfl_xor_sync(0xffffffffu, ss, o);
     }
-    const float mean = s * (1.f / C);
-    const float rstd = rsqrtf(fmaxf(ss * (1.f / C) - mean * mean, 0.f) + eps);
+    // plain form E[x^2] - mean^2 (explicit roundings, as it always computed); it cancels in fp32 when |mean| >> std, so
+    // beyond E[x^2] = 8 var (3 bits lost) a second pass over the registers computes sum (x - mean)^2
+    const float mean = __fmul_rn(s, 1.f / C);
+    float var = fmaxf(__fmaf_rn(ss, 1.f / C, -__fmul_rn(mean, mean)), 0.f);
+    // the lanes of a row hold the same s, ss and choice; the whole warp runs the second pass if any of its rows needs it
+    // (the shuffles need every lane), each row keeps its own choice
+    const bool two_pass = __fmul_rn(mean, mean) > 7.f * var;
+    if (__any_sync(0xffffffffu, two_pass)) {
+        float sd = 0.f;
+#pragma unroll
+        for (int i = 0; i < NV; ++i) {
+            const __half2* h = reinterpret_cast<const __half2*>(&v[i]);
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+                const float2 f = __half22float2(h[j]);
+                sd = fmaf(f.x - mean, f.x - mean, fmaf(f.y - mean, f.y - mean, sd));
+            }
+        }
+#pragma unroll
+        for (int o = LPR / 2; o; o >>= 1) sd += __shfl_xor_sync(0xffffffffu, sd, o);
+        if (two_pass) var = sd * (1.f / C);
+    }
+    const float rstd = rsqrtf(var + eps);
     if (!ok) return;
     uint4* yr = reinterpret_cast<uint4*>(y + static_cast<size_t>(row) * C);
     const uint4* g4 = reinterpret_cast<const uint4*>(gamma);
@@ -290,8 +390,9 @@ __global__ void k_geglu(const __half* __restrict__ x, size_t rows, int inner, __
         const __half2* xr = reinterpret_cast<const __half2*>(x + r * 2 * inner);
         const float2 h = __half22float2(xr[c2]);
         const float2 g = __half22float2(xr[inner / 2 + c2]);
-        const float g0 = 0.5f * g.x * (1.f + erff(g.x * 0.70710678118654752f));  // exact (erf) GELU
-        const float g1 = 0.5f * g.y * (1.f + erff(g.y * 0.70710678118654752f));
+        // exact (erf) GELU as g * 0.5 erfc(-g / sqrt 2): 1 + erf(g / sqrt 2) cancels for g < -3 (off by 2e-3 relative)
+        const float g0 = 0.5f * g.x * erfcf(g.x * -0.70710678118654752f);
+        const float g1 = 0.5f * g.y * erfcf(g.y * -0.70710678118654752f);
         reinterpret_cast<__half2*>(y + r * inner)[c2] = __floats2half2_rn(h.x * g0, h.y * g1);
     }
 }
@@ -576,11 +677,13 @@ __global__ void k_cfg_pndm_step(const __half* __restrict__ eps_pair, size_t n, f
         const __half gd = __float2half_rn(__half2float(d) * guidance);
         const __half e0 = __hadd(eu, gd);
         if (eps_out) eps_out[i] = e0;
-        float e = c0 * __half2float(e0);
-        if (h1) e += c1 * __half2float(h1[i]);
-        if (h2) e += c2 * __half2float(h2[i]);
-        if (h3) e += c3 * __half2float(h3[i]);
-        prev_sample[i] = __float2half_rn(ca * __half2float(sample[i]) - cb * e);
+        // explicit roundings and order: with the multiply-adds left to the compiler, the loop versions with and without
+        // eps_out contracted differently and prev came out one fp16 ulp apart depending on whether eps_out was requested
+        float e = __fmul_rn(c0, __half2float(e0));
+        if (h1) e = __fmaf_rn(c1, __half2float(h1[i]), e);
+        if (h2) e = __fmaf_rn(c2, __half2float(h2[i]), e);
+        if (h3) e = __fmaf_rn(c3, __half2float(h3[i]), e);
+        prev_sample[i] = __float2half_rn(__fmaf_rn(ca, __half2float(sample[i]), -__fmul_rn(cb, e)));
     }
 }
 
@@ -722,7 +825,7 @@ inline unsigned grid_for(size_t n, int block) {
 
 extern "C" size_t rf_group_norm_scratch_floats(int B, int HW, int groups) {
     const int nslabs = (HW + 31) / 32;
-    return static_cast<size_t>(B) * groups * 2 * (static_cast<size_t>(nslabs) + 1);
+    return static_cast<size_t>(B) * groups * 4 * (static_cast<size_t>(nslabs) + 1);
 }
 
 extern "C" int rf_group_norm_f16(const void* x, int B, int HW, int C, int groups, const void* gamma, const void* beta,
@@ -745,21 +848,24 @@ extern "C" int rf_group_norm_cat_f16(const void* x, const void* x2, int C1, int 
     const int C8 = C / 8;
     const int PPI = C8 >= 256 ? 1 : 256 / C8;
     const int threads = PPI * C8;
+    if (groups > 64 || threads < groups) return rf_fail(RF_ERR_UNSUPPORTED, "rf_group_norm_f16: at most 64 groups (and not more groups than threads)");
     // slab: >= 32 pixels (the scratch is sized for HW/32 slabs); large images take longer slabs (still >= 4 waves)
     int slab = 32;
     while (slab < 256 && static_cast<long>(B) * (HW / (2 * slab)) >= 4 * 132) slab *= 2;
     const int nslabs = (HW + slab - 1) / slab;
-    float* part = d_scratch + static_cast<size_t>(B) * groups * 2;     // [B][nslabs][G][2]
-    const size_t smem = static_cast<size_t>(PPI) * (C / 2) * sizeof(float2);
+    // d_scratch: [B][G] pivots (in B * G * 2 floats), then the plain and the shifted partials, [B][nslabs][G][2] each
+    float* part = d_scratch + static_cast<size_t>(B) * groups * 2;
+    float* part_shift = part + static_cast<size_t>(B) * nslabs * groups * 2;
+    const size_t smem = static_cast<size_t>(PPI) * (C / 2) * sizeof(float4);
     dim3 grid(nslabs, B);
     RF_LAUNCH_PDL("k_gn_partial_v", k_gn_partial_v, grid, dim3(threads), smem, st, grid.x * grid.y <= 600u, static_cast<const __half*>(x),
-                  static_cast<const __half*>(x2), C1, HW, C, groups, slab, nslabs, part);
-    if (groups > 64 || threads < groups) return rf_fail(RF_ERR_UNSUPPORTED, "rf_group_norm_f16: at most 64 groups (and not more groups than threads)");
+                  static_cast<const __half*>(x2), C1, HW, C, groups, slab, nslabs, part, part_shift, d_scratch);
     // tanh form by default: measured on the full-size UNet, both forms leave the kernels AT the fp16-storage floor
     // (1.420e-3 vs 1.418e-3 from the fp32 oracle) and the exp form costs +0.4 ms per evaluation at batch 64
     static const int silu_form = getenv("RF_SILU_EXACT") ? 1 : 2;
     RF_LAUNCH_PDL("k_gn_apply_v", k_gn_apply_v, grid, dim3(threads), size_t(0), st, grid.x * grid.y <= 600u, static_cast<const __half*>(x),
-                  static_cast<const __half*>(x2), C1, static_cast<const float*>(part), nslabs,
+                  static_cast<const __half*>(x2), C1, static_cast<const float*>(part), static_cast<const float*>(part_shift),
+                  static_cast<const float*>(d_scratch), nslabs,
                   1.f / (static_cast<float>(HW) * (C / groups)), eps, static_cast<const __half*>(gamma),
                   static_cast<const __half*>(beta), HW, C, groups, act ? silu_form : 0, slab, static_cast<__half*>(y));
     return RF_OK;
