@@ -161,7 +161,7 @@ int rf_wave_to_int16(const float* d_wave, int channels, int L, int normalize, in
                      float* d_scratch, void* stream);
 
 
-/* ==== path (b): tensor-core building blocks (tcgen05 / TMEM / TMA) ========================
+/* ==== path (b): tensor-core building blocks (wgmma / TMA) ==================================
  * The reference reaches these through diffusers' UNet2DConditionModel / AutoencoderKL forward
  * (riffusion/riffusion_pipeline.py:255,406-408,428): torch.nn.Linear / Conv2d / attention bmm.
  * All tensors fp16, device pointers; activations are NHWC ("channels last"). */
@@ -221,13 +221,10 @@ size_t rf_conv2d_workspace_bytes(const rf_conv_desc* desc);
 /* Fused attention softmax(Q K^T * scale) V per (image, head) — diffusers CrossAttention's baddbmm/softmax/bmm
  * [restated from memory] without materialising the scores.  q [B][Nq][heads*d], k [B][Nk][heads*d],
  * vt [B][heads*d][vt_pitch] (V transposed, as produced by rf_gemm_f16 with swapped operands), out [B][Nq][heads*d];
- * fp16, d a multiple of 8 and <= 192, vt_pitch a multiple of 8 >= Nk. */
-int rf_attention_f16(const void* q, const void* k, const void* vt, void* out, int B, int heads, int Nq, int Nk,
-                     int d, int vt_pitch, float scale, void* stream);
-
-/* Same with an optional causal mask (key j visible to query i iff j <= i): transformers CLIPTextModel's self-attention
- * (causal_attention_mask), the text encoder behind RiffusionPipeline.embed_text (riffusion/riffusion_pipeline.py:177-191).
- * causal != 0 requires Nk <= 128 and d <= 112. */
+ * fp16, d a multiple of 8 and <= 192, vt_pitch a multiple of 8 >= Nk.
+ * causal != 0 adds a causal mask (key j visible to query i iff j <= i): transformers CLIPTextModel's self-attention
+ * (causal_attention_mask), the text encoder behind RiffusionPipeline.embed_text (riffusion/riffusion_pipeline.py:177-191);
+ * it requires Nk <= 128 and d <= 112. */
 int rf_attention_masked_f16(const void* q, const void* k, const void* vt, void* out, int B, int heads, int Nq, int Nk,
                             int d, int vt_pitch, float scale, int causal, void* stream);
 
@@ -240,14 +237,12 @@ int rf_tc_profile_end(double* ms_out, double* flops_out, long* launches_out);
 /* Memory-bound UNet/VAE operators (fp16 activations, fp32 statistics).  NHWC images, row-major tokens.
  * Each restates the torch op diffusers calls [diffusers 0.9, absent here: restated from memory]. */
 /* torch.nn.GroupNorm(groups, C, eps) (+ optional SiLU): x,y fp16 [B][HW][C]; d_scratch: fp32 device scratch of
- * rf_group_norm_scratch_floats(B, HW, groups) floats.  Deterministic (fixed-order reductions, no atomics). */
-size_t rf_group_norm_scratch_floats(int B, int HW, int groups);
-int rf_group_norm_f16(const void* x, int B, int HW, int C, int groups, const void* gamma, const void* beta,
-                      float eps, int act, void* y, float* d_scratch, void* stream);
-/* Same on the channel concatenation [x | x2] read in place: x [B][HW][C1], x2 [B][HW][C - C1], y [B][HW][C] — the
+ * rf_group_norm_scratch_floats(B, HW, groups) floats.  Deterministic (fixed-order reductions, no atomics).
+ * With x2 != NULL the input is the channel concatenation [x | x2] read in place: x [B][HW][C1], x2 [B][HW][C - C1] — the
  * `torch.cat([hidden_states, res_hidden_states], dim=1)` of the UNet up blocks (diffusers unet_2d_blocks.py UpBlock2D /
  * CrossAttnUpBlock2D [restated from memory]) followed by the resnet's norm1, without materialising the concatenation.
- * x2 == NULL: identical to rf_group_norm_f16. */
+ * x2 == NULL: C1 is ignored. */
+size_t rf_group_norm_scratch_floats(int B, int HW, int groups);
 int rf_group_norm_cat_f16(const void* x, const void* x2, int C1, int B, int HW, int C, int groups, const void* gamma,
                           const void* beta, float eps, int act, void* y, float* d_scratch, void* stream);
 /* torch.nn.LayerNorm(C, eps) over rows */
@@ -259,8 +254,6 @@ int rf_geglu_f16(const void* x, long rows, int inner, void* y, void* stream);
 int rf_softmax_rows_f16(const void* x, long rows, int n, int pitch, void* y, void* stream);
 /* F.interpolate(scale_factor=2, mode="nearest"): [B][H][W][C] -> [B][2H][2W][C] */
 int rf_upsample2x_f16(const void* x, int B, int H, int W, int C, void* y, void* stream);
-/* torch.cat([a, b], dim=1) for NHWC tensors: [pixels][Ca] + [pixels][Cb] -> [pixels][Ca+Cb] */
-int rf_concat_channels_f16(const void* a, const void* b, long pixels, int Ca, int Cb, void* y, void* stream);
 /* Conv2d(Cin<=8 -> Cout<=8, 1x1) on NCHW fp16 with an input pre-scale: the VAE's quant_conv / post_quant_conv
  * (and the latents / 0.18215 of riffusion_pipeline.py:427 folded into in_scale) */
 int rf_conv1x1_small_f16(const void* x_nchw, const void* w, const void* bias, int B, int Cin, int Cout, long HW,

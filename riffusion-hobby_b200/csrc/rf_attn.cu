@@ -15,8 +15,6 @@
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 
-#include <cstdlib>
-#include <mutex>
 #include <string>
 
 #include "rf_common.h"
@@ -203,43 +201,6 @@ k_flash_attn(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ C
     }
 }
 
-typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                    const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                    CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-PFN_encodeTiled get_encode2() {
-    static PFN_encodeTiled fn = nullptr;
-    static std::once_flag once;
-    std::call_once(once, [] {
-        void* sym = nullptr;
-        cudaDriverEntryPointQueryResult qres;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &sym, cudaEnableDefault, &qres) == cudaSuccess &&
-            qres == cudaDriverEntryPointSuccess)
-            fn = reinterpret_cast<PFN_encodeTiled>(sym);
-    });
-    return fn;
-}
-
-int map4(CUtensorMap* map, const void* ptr, const long dims[4], const long strides[4], const int box[4]) {
-    PFN_encodeTiled enc = get_encode2();
-    if (!enc) return rf_fail(RF_ERR_CUDA, "cuTensorMapEncodeTiled unavailable (no CUDA driver)");
-    cuuint64_t gdim[4], gstr[3];
-    cuuint32_t bx[4], es[4] = {1, 1, 1, 1};
-    for (int i = 0; i < 4; ++i) {
-        gdim[i] = static_cast<cuuint64_t>(dims[i]);
-        bx[i] = static_cast<cuuint32_t>(box[i]);
-        if (i) {
-            gstr[i - 1] = static_cast<cuuint64_t>(strides[i]) * 2;
-            if (gstr[i - 1] % 16) return rf_fail(RF_ERR_INVALID, "rf_attention_f16: stride not a multiple of 16 bytes");
-        }
-    }
-    if (reinterpret_cast<uintptr_t>(ptr) % 16) return rf_fail(RF_ERR_INVALID, "rf_attention_f16: pointer not 16-byte aligned");
-    CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(ptr), gdim, gstr, bx, es,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) return rf_fail(RF_ERR_CUDA, "cuTensorMapEncodeTiled failed: " + std::to_string(int(r)));
-    return RF_OK;
-}
-
 template <int DPAD, int NV, int NS>
 int launch_attn(const CUtensorMap& mq, const CUtensorMap& mk, const CUtensorMap& mv, const AttnParams& p, dim3 grid,
                 cudaStream_t st) {
@@ -259,11 +220,6 @@ int launch_attn(const CUtensorMap& mq, const CUtensorMap& mk, const CUtensorMap&
 }  // namespace
 
 // q: [B][Nq][heads*d], k: [B][Nk][heads*d], vt: [B][heads*d][vt_pitch] (V transposed), out: [B][Nq][heads*d]; fp16.
-extern "C" int rf_attention_f16(const void* q, const void* k, const void* vt, void* out, int B, int heads, int Nq, int Nk,
-                                int d, int vt_pitch, float scale, void* stream) {
-    return rf_attention_masked_f16(q, k, vt, out, B, heads, Nq, Nk, d, vt_pitch, scale, 0, stream);
-}
-
 extern "C" int rf_attention_masked_f16(const void* q, const void* k, const void* vt, void* out, int B, int heads, int Nq,
                                        int Nk, int d, int vt_pitch, float scale, int causal, void* stream) {
     if (causal && (Nk > 128 || d > 112))
@@ -271,22 +227,23 @@ extern "C" int rf_attention_masked_f16(const void* q, const void* k, const void*
                                            "(the 77-token text encoder)");
     if (!q || !k || !vt || !out || B <= 0 || heads <= 0 || Nq <= 0 || Nk <= 0 || d <= 0 || (d % 8) || vt_pitch < Nk ||
         (vt_pitch % 8))
-        return rf_fail(RF_ERR_INVALID, "rf_attention_f16: bad argument");
-    if (d > 192) return rf_fail(RF_ERR_UNSUPPORTED, "rf_attention_f16: head dim > 192 (use the GEMM + softmax path)");
+        return rf_fail(RF_ERR_INVALID, "rf_attention_masked_f16: bad argument");
+    if (d > 192) return rf_fail(RF_ERR_UNSUPPORTED, "rf_attention_masked_f16: head dim > 192 (use the GEMM + softmax path)");
     const long C = static_cast<long>(heads) * d;
+    const int es[4] = {1, 1, 1, 1};
     CUtensorMap mq, mk, mv;
     {
         const long dims[4] = {d, Nq, heads, B};
         const long str[4] = {1, C, d, static_cast<long>(Nq) * C};
         const int box[4] = {64, TQ, 1, 1};
-        int rc = map4(&mq, q, dims, str, box);
+        int rc = rf_tma_map_f16(&mq, q, dims, str, box, es);
         if (rc) return rc;
     }
     {
         const long dims[4] = {d, Nk, heads, B};
         const long str[4] = {1, C, d, static_cast<long>(Nk) * C};
         const int box[4] = {64, TK, 1, 1};
-        int rc = map4(&mk, k, dims, str, box);
+        int rc = rf_tma_map_f16(&mk, k, dims, str, box, es);
         if (rc) return rc;
     }
     // must equal the NV template argument of the kernel variant chosen below (the TMA box defines the bytes per stage)
@@ -295,7 +252,7 @@ extern "C" int rf_attention_masked_f16(const void* q, const void* k, const void*
         const long dims[4] = {Nk, d, heads, B};
         const long str[4] = {1, vt_pitch, static_cast<long>(d) * vt_pitch, C * vt_pitch};
         const int box[4] = {TK, NV, 1, 1};
-        int rc = map4(&mv, vt, dims, str, box);
+        int rc = rf_tma_map_f16(&mv, vt, dims, str, box, es);
         if (rc) return rc;
     }
     AttnParams p;

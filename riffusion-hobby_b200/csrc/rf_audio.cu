@@ -1044,19 +1044,28 @@ static int gl_prepare_angles(rf_plan* p, const gl_ws& w, const void* d_init_angl
     return RF_OK;
 }
 
-extern "C" int rf_griffinlim(rf_plan* p, const float* d_lin, const void* d_init_angles, int B, int T,
-                             int n_iter, float momentum, float* d_wave, void* d_ws, size_t ws_bytes,
-                             void* stream) {
-    if (!p || !d_lin || !d_wave || !d_ws || B <= 0 || n_iter < 0)
-        return rf_fail(RF_ERR_INVALID, "rf_griffinlim: bad argument");
+// Prologue of the Griffin-Lim entry points `who`: argument checks, plan upload, shared-memory limits, workspace layout.
+static int gl_setup(rf_plan* p, const float* d_in, float* d_wave, void* d_ws, size_t ws_bytes, int B, int T, int n_iter,
+                    float momentum, const char* who, gl_ws* w) {
+    if (!p || !d_in || !d_wave || !d_ws || B <= 0 || n_iter < 0)
+        return rf_fail(RF_ERR_INVALID, std::string(who) + ": bad argument");
     if (!(momentum >= 0.f && momentum < 1.f))
         return rf_fail(RF_ERR_INVALID, "momentum must be in range [0, 1). Found: " + std::to_string(momentum));
-    int rc = check_T(p, T, "rf_griffinlim");
+    int rc = check_T(p, T, who);
     if (rc) return rc;
     if ((rc = rf_plan_upload(p))) return rc;
     if ((rc = set_smem_attrs())) return rc;
-    const gl_ws w = gl_layout(p, B, T, d_ws);
-    if (ws_bytes < w.total) return rf_fail(RF_ERR_INVALID, "rf_griffinlim: workspace too small");
+    *w = gl_layout(p, B, T, d_ws);
+    if (ws_bytes < w->total) return rf_fail(RF_ERR_INVALID, std::string(who) + ": workspace too small");
+    return RF_OK;
+}
+
+extern "C" int rf_griffinlim(rf_plan* p, const float* d_lin, const void* d_init_angles, int B, int T,
+                             int n_iter, float momentum, float* d_wave, void* d_ws, size_t ws_bytes,
+                             void* stream) {
+    gl_ws w;
+    int rc = gl_setup(p, d_lin, d_wave, d_ws, ws_bytes, B, T, n_iter, momentum, "rf_griffinlim", &w);
+    if (rc) return rc;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const rf_plan_host& h = p->h;
     dim3 grid((h.n_live + 31) / 32, (T + 31) / 32, B), blk(32, 32);
@@ -1066,23 +1075,23 @@ extern "C" int rf_griffinlim(rf_plan* p, const float* d_lin, const void* d_init_
     return gl_loop(p, w, B, T, n_iter, momentum, d_wave, st);
 }
 
+// inverse mel + Griffin-Lim; `prof` (optional) receives CUDA events around the loop's kernels
+static int mel_to_wave(rf_plan* p, const float* d_mel, const void* d_init_angles, int B, int T, int n_iter,
+                       float momentum, float* d_wave, void* d_ws, size_t ws_bytes, cudaStream_t st, const char* who,
+                       gl_prof* prof) {
+    gl_ws w;
+    int rc = gl_setup(p, d_mel, d_wave, d_ws, ws_bytes, B, T, n_iter, momentum, who, &w);
+    if (rc) return rc;
+    if ((rc = launch_inverse_mel(p, d_mel, B, T, 0, w.S, st))) return rc;
+    if ((rc = gl_prepare_angles(p, w, d_init_angles, B, T, st))) return rc;
+    return gl_loop(p, w, B, T, n_iter, momentum, d_wave, st, prof);
+}
+
 extern "C" int rf_mel_to_wave(rf_plan* p, const float* d_mel, const void* d_init_angles, int B, int T,
                               int n_iter, float momentum, float* d_wave, void* d_ws, size_t ws_bytes,
                               void* stream) {
-    if (!p || !d_mel || !d_wave || !d_ws || B <= 0 || n_iter < 0)
-        return rf_fail(RF_ERR_INVALID, "rf_mel_to_wave: bad argument");
-    if (!(momentum >= 0.f && momentum < 1.f))
-        return rf_fail(RF_ERR_INVALID, "momentum must be in range [0, 1). Found: " + std::to_string(momentum));
-    int rc = check_T(p, T, "rf_mel_to_wave");
-    if (rc) return rc;
-    if ((rc = rf_plan_upload(p))) return rc;
-    if ((rc = set_smem_attrs())) return rc;
-    const gl_ws w = gl_layout(p, B, T, d_ws);
-    if (ws_bytes < w.total) return rf_fail(RF_ERR_INVALID, "rf_mel_to_wave: workspace too small");
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    if ((rc = launch_inverse_mel(p, d_mel, B, T, 0, w.S, st))) return rc;
-    if ((rc = gl_prepare_angles(p, w, d_init_angles, B, T, st))) return rc;
-    return gl_loop(p, w, B, T, n_iter, momentum, d_wave, st);
+    return mel_to_wave(p, d_mel, d_init_angles, B, T, n_iter, momentum, d_wave, d_ws, ws_bytes,
+                       static_cast<cudaStream_t>(stream), "rf_mel_to_wave", nullptr);
 }
 
 // Same as rf_mel_to_wave, with every Griffin-Lim kernel launch bracketed by CUDA events on
@@ -1092,19 +1101,11 @@ extern "C" int rf_mel_to_wave(rf_plan* p, const float* d_mel, const void* d_init
 extern "C" int rf_mel_to_wave_profiled(rf_plan* p, const float* d_mel, const void* d_init_angles, int B, int T,
                                        int n_iter, float momentum, float* d_wave, void* d_ws, size_t ws_bytes,
                                        void* stream, float* ms_out, int* launches_out) {
-    if (!p || !d_mel || !d_wave || !d_ws || !ms_out || !launches_out || B <= 0 || n_iter < 0)
-        return rf_fail(RF_ERR_INVALID, "rf_mel_to_wave_profiled: bad argument");
-    int rc = check_T(p, T, "rf_mel_to_wave_profiled");
-    if (rc) return rc;
-    if ((rc = rf_plan_upload(p))) return rc;
-    if ((rc = set_smem_attrs())) return rc;
-    const gl_ws w = gl_layout(p, B, T, d_ws);
-    if (ws_bytes < w.total) return rf_fail(RF_ERR_INVALID, "rf_mel_to_wave_profiled: workspace too small");
+    if (!ms_out || !launches_out) return rf_fail(RF_ERR_INVALID, "rf_mel_to_wave_profiled: bad argument");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    if ((rc = launch_inverse_mel(p, d_mel, B, T, 0, w.S, st))) return rc;
-    if ((rc = gl_prepare_angles(p, w, d_init_angles, B, T, st))) return rc;
     gl_prof prof;
-    rc = gl_loop(p, w, B, T, n_iter, momentum, d_wave, st, &prof);
+    const int rc = mel_to_wave(p, d_mel, d_init_angles, B, T, n_iter, momentum, d_wave, d_ws, ws_bytes, st,
+                               "rf_mel_to_wave_profiled", &prof);
     cudaError_t e = cudaStreamSynchronize(st);
     for (int c = 0; c < 3; ++c) {
         ms_out[c] = 0.f;
@@ -1238,7 +1239,7 @@ extern "C" int rf_mel_to_image(const float* d_mel, int channels, int height, int
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     RF_CUDA_TRY(cudaMemsetAsync(d_max, 0, 4, st));
     const size_t n = static_cast<size_t>(channels) * height * width;
-    k_absmax<<<296, 256, 0, st>>>(d_mel, n, 0, d_max);
+    k_absmax<<<2 * rf_num_sms(), 256, 0, st>>>(d_mel, n, 0, d_max);
     RF_CUDA_LAUNCH_CHECK("k_absmax");
     dim3 grid((width + 127) / 128, height);
     k_mel_to_image<<<grid, 128, 0, st>>>(d_mel, channels, height, width, power, d_max, d_img);
@@ -1253,7 +1254,7 @@ extern "C" int rf_wave_to_int16(const float* d_wave, int channels, int L, int no
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     if (normalize) {
         RF_CUDA_TRY(cudaMemsetAsync(d_scratch, 0, 4, st));
-        k_absmax<<<296, 256, 0, st>>>(d_wave, static_cast<size_t>(channels) * L, 1, d_scratch);
+        k_absmax<<<2 * rf_num_sms(), 256, 0, st>>>(d_wave, static_cast<size_t>(channels) * L, 1, d_scratch);
         RF_CUDA_LAUNCH_CHECK("k_absmax");
     }
     k_wave_to_int16<<<(L + 255) / 256, 256, 0, st>>>(d_wave, channels, L, d_scratch, normalize, d_pcm);

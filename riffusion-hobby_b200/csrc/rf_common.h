@@ -1,4 +1,4 @@
-// Error plumbing shared by the C-ABI translation units.
+// Error plumbing and per-device launch state shared by the C-ABI translation units.
 #pragma once
 #include <cuda_runtime.h>
 
@@ -42,6 +42,19 @@ inline cudaError_t rf_set_smem_once(rf_dev_once& o, F* func, int bytes) {
     e = cudaFuncSetAttribute(func, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
     if (e == cudaSuccess) o.done.fetch_or(bit, std::memory_order_release);
     return e;
+}
+
+// SM count of the current device, cached per device like rf_set_smem_once (up to 64 devices); 132, the H100 SXM's count,
+// if the query fails.  Launch geometries scale with it.
+inline int rf_num_sms() {
+    static std::atomic<int> cached[64];
+    int dev = 0, n = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess) return 132;
+    std::atomic<int>& c = cached[dev & 63];
+    if ((n = c.load(std::memory_order_relaxed))) return n;
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) return 132;
+    c.store(n, std::memory_order_relaxed);
+    return n;
 }
 
 

@@ -408,47 +408,6 @@ k_tc_gemm(const __grid_constant__ CUtensorMap mapA0, const __grid_constant__ CUt
 }
 
 // ------------------------------------------------------------------------------ host side
-typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                    const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                    CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-PFN_encodeTiled get_encode() {
-    static PFN_encodeTiled fn = nullptr;
-    static std::once_flag once;
-    std::call_once(once, [] {
-        void* sym = nullptr;
-        cudaDriverEntryPointQueryResult qres;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &sym, cudaEnableDefault, &qres) == cudaSuccess &&
-            qres == cudaDriverEntryPointSuccess)
-            fn = reinterpret_cast<PFN_encodeTiled>(sym);
-    });
-    return fn;
-}
-
-// fp16 tensor map, rank 4, dims/strides innermost first (strides in elements; stride[0] must be 1)
-int make_map(CUtensorMap* map, const void* ptr, const long dims[4], const long strides[4], const int box[4],
-             const int estrides[4]) {
-    PFN_encodeTiled enc = get_encode();
-    if (!enc) return rf_fail(RF_ERR_CUDA, "cuTensorMapEncodeTiled unavailable (no CUDA driver)");
-    cuuint64_t gdim[4], gstr[3];
-    cuuint32_t bx[4], es[4];
-    for (int i = 0; i < 4; ++i) {
-        gdim[i] = static_cast<cuuint64_t>(dims[i]);
-        bx[i] = static_cast<cuuint32_t>(box[i]);
-        es[i] = static_cast<cuuint32_t>(estrides[i]);
-        if (i) {
-            gstr[i - 1] = static_cast<cuuint64_t>(strides[i]) * 2;
-            if (gstr[i - 1] % 16) return rf_fail(RF_ERR_INVALID, "tensor map: stride not a multiple of 16 bytes");
-        }
-    }
-    if (reinterpret_cast<uintptr_t>(ptr) % 16) return rf_fail(RF_ERR_INVALID, "tensor map: base not 16-byte aligned");
-    CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(ptr), gdim, gstr, bx, es,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) return rf_fail(RF_ERR_CUDA, "cuTensorMapEncodeTiled failed: " + std::to_string(int(r)));
-    return RF_OK;
-}
-
 // optional live measurement (bench.py): CUDA events around every tensor-core launch + algorithmic FLOP count
 struct TcProfile {
     bool on = false;
@@ -458,15 +417,6 @@ struct TcProfile {
     struct Rec { int conv, M, N, K, batch, splits, bn; };   // bn < 0: CTA-pair kernel
     std::vector<Rec> recs;
 };
-int num_sms_cached() {
-    static int n = 0;
-    if (!n) {
-        int dev = 0;
-        if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess)
-            n = 132;
-    }
-    return n;
-}
 
 TcProfile g_prof;
 std::mutex g_prof_mu;
@@ -477,7 +427,7 @@ int launch(const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& b, c
     constexpr size_t smem = static_cast<size_t>(STAGES) * A_TILE_BYTES +
                             static_cast<size_t>(BRES ? BRES_KB : STAGES) * (BN * BK * 2) + stage_bytes(BN) + 1024;
     static_assert(smem <= 232448, "shared memory budget (227 KB per block)");
-    const int num_sms = num_sms_cached();
+    const int num_sms = rf_num_sms();
     const int n_tiles = static_cast<int>(grid.x * grid.y * grid.z);
     if (BRES) {   // every CTA is bound to one column block: a multiple of tiles_n CTAs
         grid = dim3(static_cast<unsigned>((num_sms / p.tiles_n) * p.tiles_n));
@@ -594,7 +544,7 @@ int pick_bn(int N, long tiles_m) {
     }
     if (N <= 64) return 64;
     if (N % 160) return 128;
-    const long sms = num_sms_cached();
+    const long sms = rf_num_sms();
     const long t128 = tiles_m * ((N + 127) / 128), t160 = tiles_m * (N / 160);
     const long c128 = ((t128 + sms - 1) / sms) * 128, c160 = ((t160 + sms - 1) / sms) * 160;
     return c160 * 100 <= c128 * 102 ? 160 : 128;
@@ -610,7 +560,7 @@ int dispatch(int N, int bn, const CUtensorMap& a0, const CUtensorMap& a1, const 
     const bool can_split = nbatch == 1 && p.act != 2 && (N % 8) == 0 && (p.ldo % 8) == 0 && (!p.conv || p.osx == 1) &&
                            (!p.residual || (p.ldr % 8) == 0) &&
                            ((reinterpret_cast<uintptr_t>(p.out ? static_cast<void*>(p.out) : static_cast<void*>(p.out_f32)) & 15) == 0);
-    p.splits = pick_splits(rows, N, p.tiles_n * tiles_m, p.num_kb, num_sms_cached(), can_split);
+    p.splits = pick_splits(rows, N, p.tiles_n * tiles_m, p.num_kb, rf_num_sms(), can_split);
     p.kb_per_split = (p.num_kb + p.splits - 1) / p.splits;
     p.ws = nullptr;
     p.ws_split_stride = rows * N;
@@ -635,7 +585,7 @@ int dispatch(int N, int bn, const CUtensorMap& a0, const CUtensorMap& a1, const 
     int rc;
     const char* env_bres = getenv("RF_GEMM_BRES");
     if (bn == 160 && nbatch == 1 && p.splits == 1 && p.num_kb <= BRES_KB && p.tiles_n <= 8 &&
-        static_cast<long>(tiles_m) * p.tiles_n >= 4L * num_sms_cached() && !(env_bres && env_bres[0] == '0')) {
+        static_cast<long>(tiles_m) * p.tiles_n >= 4L * rf_num_sms() && !(env_bres && env_bres[0] == '0')) {
         return launch<160, 2, true>(a0, a1, b, p, grid, st);       // B-stationary (K <= 320, N = 160 k)
     }
     if (bn == 160) rc = launch<160, 3>(a0, a1, b, p, grid, st);   // N = 320-type layers: two exact 160-column tiles
@@ -643,7 +593,7 @@ int dispatch(int N, int bn, const CUtensorMap& a0, const CUtensorMap& a1, const 
     else rc = launch<64, 6>(a0, a1, b, p, grid, st);
     if (rc || p.splits == 1) return rc;
     const long work = rows * (N / 8);
-    const unsigned blocks = static_cast<unsigned>(std::min<long>((work + 255) / 256, 8L * num_sms_cached()));
+    const unsigned blocks = static_cast<unsigned>(std::min<long>((work + 255) / 256, 8L * rf_num_sms()));
     k_splitk_reduce<<<blocks, 256, 0, st>>>(p.ws, p.splits, p.ws_split_stride, rows, N, p.ldo, p.ldr,
                                             p.conv ? p.Ho * p.Wo : 1, p.alpha, p.bias, p.bias_mode, p.bias2, p.bias2_pitch,
                                             p.act, p.residual, p.out, p.out_f32);
@@ -656,6 +606,46 @@ int dispatch(int N, int bn, const CUtensorMap& a0, const CUtensorMap& a1, const 
 }
 
 }  // namespace
+
+typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
+                                    const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
+                                    CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+
+static PFN_encodeTiled get_encode() {
+    static PFN_encodeTiled fn = nullptr;
+    static std::once_flag once;
+    std::call_once(once, [] {
+        void* sym = nullptr;
+        cudaDriverEntryPointQueryResult qres;
+        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &sym, cudaEnableDefault, &qres) == cudaSuccess &&
+            qres == cudaDriverEntryPointSuccess)
+            fn = reinterpret_cast<PFN_encodeTiled>(sym);
+    });
+    return fn;
+}
+
+int rf_tma_map_f16(CUtensorMap* map, const void* ptr, const long dims[4], const long strides[4], const int box[4],
+                   const int estrides[4]) {
+    PFN_encodeTiled enc = get_encode();
+    if (!enc) return rf_fail(RF_ERR_CUDA, "cuTensorMapEncodeTiled unavailable (no CUDA driver)");
+    cuuint64_t gdim[4], gstr[3];
+    cuuint32_t bx[4], es[4];
+    for (int i = 0; i < 4; ++i) {
+        gdim[i] = static_cast<cuuint64_t>(dims[i]);
+        bx[i] = static_cast<cuuint32_t>(box[i]);
+        es[i] = static_cast<cuuint32_t>(estrides[i]);
+        if (i) {
+            gstr[i - 1] = static_cast<cuuint64_t>(strides[i]) * 2;
+            if (gstr[i - 1] % 16) return rf_fail(RF_ERR_INVALID, "tensor map: stride not a multiple of 16 bytes");
+        }
+    }
+    if (reinterpret_cast<uintptr_t>(ptr) % 16) return rf_fail(RF_ERR_INVALID, "tensor map: base not 16-byte aligned");
+    CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(ptr), gdim, gstr, bx, es,
+                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) return rf_fail(RF_ERR_CUDA, "cuTensorMapEncodeTiled failed: " + std::to_string(int(r)));
+    return RF_OK;
+}
 
 // ------------------------------------------------------------------------------ C-ABI
 static int gemm_impl(const rf_gemm_desc* d, void* stream, size_t* query) {
@@ -671,7 +661,7 @@ static int gemm_impl(const rf_gemm_desc* d, void* stream, size_t* query) {
         const long str[4] = {1, d->lda, a_m1 ? d->sa1 : d->lda, a_m2 ? d->sa2 : d->lda};
         const int box[4] = {BK, BM, 1, 1};
         const int es[4] = {1, 1, 1, 1};
-        int rc = make_map(&ma, d->A, dims, str, box, es);
+        int rc = rf_tma_map_f16(&ma, d->A, dims, str, box, es);
         if (rc) return rc;
     }
     const int bn = pick_bn(d->N, static_cast<long>((d->M + BM - 1) / BM) * b1 * b2);
@@ -680,7 +670,7 @@ static int gemm_impl(const rf_gemm_desc* d, void* stream, size_t* query) {
         const long str[4] = {1, d->ldb, b_m1 ? d->sb1 : d->ldb, b_m2 ? d->sb2 : d->ldb};
         const int box[4] = {BK, bn, 1, 1};
         const int es[4] = {1, 1, 1, 1};
-        int rc = make_map(&mb, d->B, dims, str, box, es);
+        int rc = rf_tma_map_f16(&mb, d->B, dims, str, box, es);
         if (rc) return rc;
     }
     TcParams p{};
@@ -744,7 +734,7 @@ static int conv_impl(const rf_conv_desc* d, void* stream, size_t* query) {
         const long str[4] = {1, d->C1, static_cast<long>(d->W) * d->C1, static_cast<long>(d->H) * d->W * d->C1};
         const int box[4] = {BK, (bw - 1) * s + 1, (bh - 1) * s + 1, bb};
         const int es[4] = {1, s, s, 1};
-        int rc = make_map(&m1, d->x1, dims, str, box, es);
+        int rc = rf_tma_map_f16(&m1, d->x1, dims, str, box, es);
         if (rc) return rc;
     }
     m2 = m1;
@@ -753,7 +743,7 @@ static int conv_impl(const rf_conv_desc* d, void* stream, size_t* query) {
         const long str[4] = {1, C2, static_cast<long>(d->W) * C2, static_cast<long>(d->H) * d->W * C2};
         const int box[4] = {BK, (bw - 1) * s + 1, (bh - 1) * s + 1, bb};
         const int es[4] = {1, s, s, 1};
-        int rc = make_map(&m2, d->x2, dims, str, box, es);
+        int rc = rf_tma_map_f16(&m2, d->x2, dims, str, box, es);
         if (rc) return rc;
     }
     const int taps = d->ksize * d->ksize;
@@ -765,7 +755,7 @@ static int conv_impl(const rf_conv_desc* d, void* stream, size_t* query) {
         const long str[4] = {1, Ktot, Ktot * d->Cout, Ktot * d->Cout};
         const int box[4] = {BK, bn, 1, 1};
         const int es[4] = {1, 1, 1, 1};
-        int rc = make_map(&mb, d->w, dims, str, box, es);
+        int rc = rf_tma_map_f16(&mb, d->w, dims, str, box, es);
         if (rc) return rc;
     }
     TcParams p{};
@@ -811,7 +801,7 @@ static int conv_impl(const rf_conv_desc* d, void* stream, size_t* query) {
         const long str[4] = {1, Ktot, Ktot * d->Cout, Ktot * d->Cout};
         const int box[4] = {BK, bn, 1, 1};
         const int es[4] = {1, 1, 1, 1};
-        int rc = make_map(&mph, static_cast<const __half*>(d->w) + static_cast<long>(ph) * d->Cout * Ktot, dims, str, box, es);
+        int rc = rf_tma_map_f16(&mph, static_cast<const __half*>(d->w) + static_cast<long>(ph) * d->Cout * Ktot, dims, str, box, es);
         if (rc) return rc;
         TcParams q = p;
         rc = dispatch(d->Cout, bn, m1, m2, mph, q, p.tiles_x * p.tiles_y * tiles_b, 1, static_cast<cudaStream_t>(stream), nullptr, 0,

@@ -81,3 +81,9 @@ __device__ __forceinline__ void reg_fence(float* d) {
 #include "rf_wgmma.inc"
 
 }  // namespace tc
+
+// Host: encodes an fp16 rank-4 tensor map with 128-byte swizzle, the layout the descriptors above expect.  dims, strides,
+// box and element strides are innermost first; strides are in elements and strides[0] must be 1.  Returns RF_OK or the
+// rf_fail code (defined in rf_gemm.cu).
+int rf_tma_map_f16(CUtensorMap* map, const void* ptr, const long dims[4], const long strides[4], const int box[4],
+                   const int estrides[4]);

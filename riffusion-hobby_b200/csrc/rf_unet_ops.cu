@@ -702,22 +702,6 @@ __global__ void k_axpby(const __half* __restrict__ x, const __half* __restrict__
     }
 }
 
-// channel concatenation of two NHWC tensors (torch.cat([a, b], dim=1) in NCHW terms)
-__global__ void k_concat_channels(const __half* __restrict__ a, const __half* __restrict__ b, size_t pixels, int Ca,
-                                  int Cb, __half* __restrict__ y) {
-    const int C8 = (Ca + Cb) / 8, A8 = Ca / 8;
-    const size_t n = pixels * C8;
-    const uint4* as = reinterpret_cast<const uint4*>(a);
-    const uint4* bs = reinterpret_cast<const uint4*>(b);
-    uint4* ys = reinterpret_cast<uint4*>(y);
-    for (size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < n;
-         i += static_cast<size_t>(gridDim.x) * blockDim.x) {
-        const size_t p = i / C8;
-        const int c = static_cast<int>(i % C8);
-        ys[i] = c < A8 ? as[p * A8 + c] : bs[p * (Cb / 8) + (c - A8)];
-    }
-}
-
 // 1x1 convolution on tiny channel counts, NCHW: y[b][o][p] = bias[o] + sum_i w[o][i] * (in_scale * x[b][i][p])
 __global__ void k_conv1x1_small(const __half* __restrict__ x, const __half* __restrict__ w, const __half* __restrict__ bias,
                                 int B, int Cin, int Cout, size_t HW, float in_scale, __half* __restrict__ y) {
@@ -816,9 +800,10 @@ __global__ void k_slerp_apply(const __half* __restrict__ v0, const __half* __res
         out[b * n + i] = __float2half_rn(s0 * __half2float(v0[b * n + i]) + s1 * __half2float(v1[b * n + i]));
 }
 
+// grid of a grid-stride loop: at most 16 CTAs per SM
 inline unsigned grid_for(size_t n, int block) {
-    size_t g = (n + block - 1) / block;
-    return static_cast<unsigned>(g > 132 * 16 ? 132 * 16 : (g ? g : 1));
+    const size_t g = (n + block - 1) / block, cap = static_cast<size_t>(rf_num_sms()) * 16;
+    return static_cast<unsigned>(g > cap ? cap : (g ? g : 1));
 }
 
 }  // namespace
@@ -828,30 +813,26 @@ extern "C" size_t rf_group_norm_scratch_floats(int B, int HW, int groups) {
     return static_cast<size_t>(B) * groups * 4 * (static_cast<size_t>(nslabs) + 1);
 }
 
-extern "C" int rf_group_norm_f16(const void* x, int B, int HW, int C, int groups, const void* gamma, const void* beta,
-                                 float eps, int act, void* y, float* d_scratch, void* stream) {
-    return rf_group_norm_cat_f16(x, nullptr, C, B, HW, C, groups, gamma, beta, eps, act, y, d_scratch, stream);
-}
-
 extern "C" int rf_group_norm_cat_f16(const void* x, const void* x2, int C1, int B, int HW, int C, int groups,
                                      const void* gamma, const void* beta, float eps, int act, void* y, float* d_scratch,
                                      void* stream) {
     if (!x || !y || !gamma || !beta || !d_scratch || B <= 0 || HW <= 0 || C <= 0 || groups <= 0 || C % groups ||
         ((C / groups) & 1))
-        return rf_fail(RF_ERR_INVALID, "rf_group_norm_f16: bad argument (channels per group must be even)");
+        return rf_fail(RF_ERR_INVALID, "rf_group_norm_cat_f16: bad argument (channels per group must be even)");
     if (!x2) C1 = C;
     if (x2 && (C1 <= 0 || C1 >= C || (C1 % 8) || ((C - C1) % 8)))
         return rf_fail(RF_ERR_INVALID, "rf_group_norm_cat_f16: both channel counts must be positive multiples of 8");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    if (C > 2560 || (C % 8)) return rf_fail(RF_ERR_UNSUPPORTED, "rf_group_norm_f16: C must be a multiple of 8, <= 2560");
+    if (C > 2560 || (C % 8)) return rf_fail(RF_ERR_UNSUPPORTED, "rf_group_norm_cat_f16: C must be a multiple of 8, <= 2560");
     // thread -> (pixel phase, 8-channel column): blockDim = PPI * C/8 (<= 320 threads)
     const int C8 = C / 8;
     const int PPI = C8 >= 256 ? 1 : 256 / C8;
     const int threads = PPI * C8;
-    if (groups > 64 || threads < groups) return rf_fail(RF_ERR_UNSUPPORTED, "rf_group_norm_f16: at most 64 groups (and not more groups than threads)");
-    // slab: >= 32 pixels (the scratch is sized for HW/32 slabs); large images take longer slabs (still >= 4 waves)
+    if (groups > 64 || threads < groups) return rf_fail(RF_ERR_UNSUPPORTED, "rf_group_norm_cat_f16: at most 64 groups (and not more groups than threads)");
+    // slab: >= 32 pixels (the scratch is sized for HW/32 slabs); large images take longer slabs (still >= 4 waves).
+    // The slab length sets the summation order: devices with different SM counts may differ in the last bits.
     int slab = 32;
-    while (slab < 256 && static_cast<long>(B) * (HW / (2 * slab)) >= 4 * 132) slab *= 2;
+    while (slab < 256 && static_cast<long>(B) * (HW / (2 * slab)) >= 4L * rf_num_sms()) slab *= 2;
     const int nslabs = (HW + slab - 1) / slab;
     // d_scratch: [B][G] pivots (in B * G * 2 floats), then the plain and the shifted partials, [B][nslabs][G][2] each
     float* part = d_scratch + static_cast<size_t>(B) * groups * 2;
@@ -923,17 +904,6 @@ extern "C" int rf_upsample2x_f16(const void* x, int B, int H, int W, int C, void
     return RF_OK;
 }
 
-extern "C" int rf_concat_channels_f16(const void* a, const void* b, long pixels, int Ca, int Cb, void* y, void* stream) {
-    if (!a || !b || !y || pixels <= 0 || Ca <= 0 || Cb <= 0 || (Ca % 8) || (Cb % 8))
-        return rf_fail(RF_ERR_INVALID, "rf_concat_channels_f16: bad argument");
-    const size_t n = static_cast<size_t>(pixels) * ((Ca + Cb) / 8);
-    k_concat_channels<<<grid_for(n, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
-        static_cast<const __half*>(a), static_cast<const __half*>(b), static_cast<size_t>(pixels), Ca, Cb,
-        static_cast<__half*>(y));
-    RF_CUDA_LAUNCH_CHECK("k_concat_channels");
-    return RF_OK;
-}
-
 extern "C" int rf_slerp_f16(const void* v0, const void* v1, int B, long n, const float* d_alphas, float dot_threshold,
                             void* out, float* d_scratch, void* stream) {
     if (!v0 || !v1 || !out || !d_alphas || !d_scratch || B <= 0 || n <= 0) return rf_fail(RF_ERR_INVALID, "rf_slerp_f16: bad argument");
@@ -972,9 +942,10 @@ template <int NCO2>
 static int launch_conv_in_blk(const void* x, const void* w, const void* bias, int B, int Cin, int H, int W, void* y,
                               cudaStream_t st) {
     const size_t smem = (static_cast<size_t>(64 * NCO2) * Cin * 9 + 8 * 18 * 8) * sizeof(float);
-    RF_CUDA_TRY(cudaFuncSetAttribute(k_conv_in_blk<NCO2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
+    static rf_dev_once once;
+    RF_CUDA_TRY(rf_set_smem_once(once, k_conv_in_blk<NCO2>, 96 * 1024));
     const long ngroups = static_cast<long>(B) * H * (W / 4);
-    const unsigned grid = static_cast<unsigned>(std::min<long>((ngroups + 7) / 8, 2 * 132));
+    const unsigned grid = static_cast<unsigned>(std::min<long>((ngroups + 7) / 8, 2L * rf_num_sms()));
     k_conv_in_blk<NCO2><<<grid, 256, smem, st>>>(static_cast<const __half*>(x), static_cast<const __half*>(w),
                                                  static_cast<const __half*>(bias), B, Cin, H, W, static_cast<__half*>(y));
     RF_CUDA_LAUNCH_CHECK("k_conv_in_blk");
@@ -994,11 +965,8 @@ extern "C" int rf_conv_in_f16(const void* x_nchw, const void* w, const void* bia
     }
     const size_t smem = static_cast<size_t>(Cout) * Cin * 9 * sizeof(float);
     if (smem > 96 * 1024) return rf_fail(RF_ERR_UNSUPPORTED, "rf_conv_in_f16: weights too large");
-    static bool attr = false;
-    if (!attr) {
-        RF_CUDA_TRY(cudaFuncSetAttribute(k_conv_in_generic, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
-        attr = true;
-    }
+    static rf_dev_once once;
+    RF_CUDA_TRY(rf_set_smem_once(once, k_conv_in_generic, 96 * 1024));
     const size_t npix = static_cast<size_t>(B) * H * W;
     k_conv_in_generic<<<static_cast<unsigned>((npix + 63) / 64), 256, smem, st>>>(
         static_cast<const __half*>(x_nchw), static_cast<const __half*>(w), static_cast<const __half*>(bias), B, Cin, H, W,
@@ -1011,9 +979,10 @@ template <int NSTEP>
 static int launch_conv_out_blk(const void* x, const void* w, const void* bias, int B, int H, int W, int Cout, void* y,
                                cudaStream_t st) {
     const size_t smem = static_cast<size_t>(9) * NSTEP * 256 * sizeof(float);
-    RF_CUDA_TRY(cudaFuncSetAttribute(k_conv_out_blk<NSTEP>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
+    static rf_dev_once once;
+    RF_CUDA_TRY(rf_set_smem_once(once, k_conv_out_blk<NSTEP>, 96 * 1024));
     const long ngroups = static_cast<long>(B) * H * (W / 4);
-    const unsigned grid = static_cast<unsigned>(std::min<long>((ngroups + 7) / 8, 2 * 132));
+    const unsigned grid = static_cast<unsigned>(std::min<long>((ngroups + 7) / 8, 2L * rf_num_sms()));
     k_conv_out_blk<NSTEP><<<grid, 256, smem, st>>>(static_cast<const __half*>(x), static_cast<const __half*>(w),
                                                    static_cast<const __half*>(bias), B, H, W, Cout, static_cast<__half*>(y));
     RF_CUDA_LAUNCH_CHECK("k_conv_out_blk");

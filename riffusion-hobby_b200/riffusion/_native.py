@@ -98,8 +98,6 @@ SIGNATURES = {
     "rf_gemm_workspace_bytes": (C.c_size_t, [C.POINTER(GemmDesc)]),
     "rf_conv2d_workspace_bytes": (C.c_size_t, [C.POINTER(ConvDesc)]),
     "rf_group_norm_scratch_floats": (C.c_size_t, [C.c_int, C.c_int, C.c_int]),
-    "rf_group_norm_f16": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_float,
-                                    C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     "rf_group_norm_cat_f16": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p,
                                         C.c_void_p, C.c_float, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     "rf_layer_norm_f16": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_float, C.c_void_p,
@@ -107,7 +105,6 @@ SIGNATURES = {
     "rf_geglu_f16": (C.c_int, [C.c_void_p, C.c_long, C.c_int, C.c_void_p, C.c_void_p]),
     "rf_softmax_rows_f16": (C.c_int, [C.c_void_p, C.c_long, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     "rf_upsample2x_f16": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
-    "rf_concat_channels_f16": (C.c_int, [C.c_void_p, C.c_void_p, C.c_long, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     "rf_conv1x1_small_f16": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_long, C.c_float,
                                        C.c_void_p, C.c_void_p]),
     "rf_vae_image_to_u8": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
@@ -124,8 +121,6 @@ SIGNATURES = {
                                        C.c_void_p]),
     "rf_axpby_f16": (C.c_int, [C.c_void_p, C.c_void_p, C.c_float, C.c_float, C.c_void_p, C.c_void_p, C.c_long,
                                C.c_void_p, C.c_void_p]),
-    "rf_attention_f16": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int,
-                                   C.c_int, C.c_int, C.c_float, C.c_void_p]),
     "rf_attention_masked_f16": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int,
                                    C.c_int, C.c_int, C.c_float, C.c_int, C.c_void_p]),
     "rf_tc_profile_begin": (C.c_int, []),
@@ -178,6 +173,13 @@ def ptr(t: torch.Tensor | None) -> int | None:
 
 def stream_ptr(device: torch.device) -> int:
     return torch.cuda.current_stream(device).cuda_stream
+
+
+def call(name: str, device: torch.device, *args) -> None:
+    """Call the entry point `name` with `args` and, as its last argument, the current stream of `device`, with `device`
+    current; a non-zero return is raised through `check`."""
+    with torch.cuda.device(device):
+        check(getattr(lib(), name)(*args, stream_ptr(device)))
 
 
 def require_cuda(t: torch.Tensor, name: str, dtype: torch.dtype) -> torch.Tensor:

@@ -334,11 +334,10 @@ class RiffusionPipeline:
         u8 = ops.vae_image_to_u8(image)
         B, H, W, _ = u8.shape
         mel = torch.empty((B, H, W), dtype=torch.float32, device=u8.device)
-        lib = _native.lib()
         p = converter.p
         for i in range(B):
-            _native.check(lib.rf_image_to_mel(u8[i].data_ptr(), H, W, 0, float(p.power_for_image), 30e6, mel[i].data_ptr(),
-                                              _native.stream_ptr(u8.device)))
+            _native.call("rf_image_to_mel", u8.device, u8[i].data_ptr(), H, W, 0, float(p.power_for_image), 30e6,
+                         mel[i].data_ptr())
         wave = converter.waveform_from_mel_amplitudes(mel, init_angles)
         return dict(images=u8, waveform=wave, latents=out["latents"], latents_unscaled=latents,
                     n_unet_evals=out["n_unet_evals"])

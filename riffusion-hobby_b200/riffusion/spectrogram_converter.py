@@ -149,9 +149,7 @@ class Spectrogram(_Transform):
         B, L = x.shape
         Tn = 1 + L // self.p.hop_length
         spec = torch.empty((B, plan.info.n_freq, Tn), dtype=torch.complex64, device=x.device)
-        with torch.cuda.device(x.device):
-            _native.check(_native.lib().rf_stft(plan.handle, x.data_ptr(), B, L, spec.data_ptr(),
-                                                _native.stream_ptr(x.device)))
+        _native.call("rf_stft", x.device, plan.handle, x.data_ptr(), B, L, spec.data_ptr())
         return spec.reshape(tuple(lead) + spec.shape[-2:])
 
 
@@ -165,9 +163,7 @@ class MelScale(_Transform):
         if F != plan.info.n_freq:
             raise ValueError(f"Expected {plan.info.n_freq} frequency bins. Found: {F}")
         mel = torch.empty((B, self.p.num_frequencies, Tn), dtype=torch.float32, device=s.device)
-        with torch.cuda.device(s.device):
-            _native.check(_native.lib().rf_mel_scale(plan.handle, s.data_ptr(), B, Tn, mel.data_ptr(),
-                                                     _native.stream_ptr(s.device)))
+        _native.call("rf_mel_scale", s.device, plan.handle, s.data_ptr(), B, Tn, mel.data_ptr())
         return mel.reshape(tuple(lead) + mel.shape[-2:])
 
 
@@ -183,9 +179,7 @@ class InverseMelScale(_Transform):
         if n_mels != self.p.num_frequencies:
             raise ValueError("Expected an input with {} mel bins. Found: {}".format(self.p.num_frequencies, n_mels))
         lin = torch.empty((B, plan.info.n_freq, Tn), dtype=torch.float32, device=m.device)
-        with torch.cuda.device(m.device):
-            _native.check(_native.lib().rf_inverse_mel(plan.handle, m.data_ptr(), B, Tn, lin.data_ptr(),
-                                                       _native.stream_ptr(m.device)))
+        _native.call("rf_inverse_mel", m.device, plan.handle, m.data_ptr(), B, Tn, lin.data_ptr())
         return lin.reshape(tuple(lead) + lin.shape[-2:])
 
 
@@ -207,12 +201,10 @@ class GriffinLim(_Transform):
             init_angles = torch.rand(s.size(), dtype=torch.complex64, device=s.device)
         ang = _native.require_cuda(init_angles, "init_angles", torch.complex64).reshape(B, F, Tn)
         wave = torch.empty((B, self.p.hop_length * (Tn - 1)), dtype=torch.float32, device=s.device)
-        with torch.cuda.device(s.device):
-            nbytes = _native.lib().rf_griffinlim_workspace_bytes(plan.handle, B, Tn)
-            ws = torch.empty(nbytes, dtype=torch.uint8, device=s.device)
-            _native.check(_native.lib().rf_griffinlim(
-                plan.handle, s.data_ptr(), ang.data_ptr(), B, Tn, self.p.num_griffin_lim_iters,
-                self.momentum, wave.data_ptr(), ws.data_ptr(), nbytes, _native.stream_ptr(s.device)))
+        nbytes = _native.lib().rf_griffinlim_workspace_bytes(plan.handle, B, Tn)
+        ws = torch.empty(nbytes, dtype=torch.uint8, device=s.device)
+        _native.call("rf_griffinlim", s.device, plan.handle, s.data_ptr(), ang.data_ptr(), B, Tn,
+                     self.p.num_griffin_lim_iters, self.momentum, wave.data_ptr(), ws.data_ptr(), nbytes)
         return wave.reshape(tuple(lead) + wave.shape[-1:])
 
 
@@ -274,9 +266,7 @@ class SpectrogramConverter:
         B, L = x.shape
         Tn = 1 + L // self.p.hop_length
         mel = torch.empty((B, self.p.num_frequencies, Tn), dtype=torch.float32, device=x.device)
-        with torch.cuda.device(x.device):
-            _native.check(_native.lib().rf_stft_mel(plan.handle, x.data_ptr(), B, L, mel.data_ptr(),
-                                                    _native.stream_ptr(x.device)))
+        _native.call("rf_stft_mel", x.device, plan.handle, x.data_ptr(), B, L, mel.data_ptr())
         return mel.reshape(tuple(lead) + mel.shape[-2:])
 
     def waveform_from_mel_amplitudes(
@@ -295,10 +285,8 @@ class SpectrogramConverter:
             init_angles = torch.rand((B, F, Tn), dtype=torch.complex64, device=m.device)
         ang = _native.require_cuda(init_angles, "init_angles", torch.complex64).reshape(B, F, Tn)
         wave = torch.empty((B, self.p.hop_length * (Tn - 1)), dtype=torch.float32, device=m.device)
-        with torch.cuda.device(m.device):
-            nbytes = _native.lib().rf_griffinlim_workspace_bytes(plan.handle, B, Tn)
-            ws = torch.empty(nbytes, dtype=torch.uint8, device=m.device)
-            _native.check(_native.lib().rf_mel_to_wave(
-                plan.handle, m.data_ptr(), ang.data_ptr(), B, Tn, self.p.num_griffin_lim_iters,
-                GriffinLim.momentum, wave.data_ptr(), ws.data_ptr(), nbytes, _native.stream_ptr(m.device)))
+        nbytes = _native.lib().rf_griffinlim_workspace_bytes(plan.handle, B, Tn)
+        ws = torch.empty(nbytes, dtype=torch.uint8, device=m.device)
+        _native.call("rf_mel_to_wave", m.device, plan.handle, m.data_ptr(), ang.data_ptr(), B, Tn,
+                     self.p.num_griffin_lim_iters, GriffinLim.momentum, wave.data_ptr(), ws.data_ptr(), nbytes)
         return wave.reshape(tuple(lead) + wave.shape[-1:])

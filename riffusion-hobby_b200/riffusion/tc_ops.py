@@ -21,10 +21,6 @@ def _f16(t: torch.Tensor, name: str) -> torch.Tensor:
     return t
 
 
-def _stream(t: torch.Tensor) -> int:
-    return torch.cuda.current_stream(t.device).cuda_stream
-
-
 def _workspace(nbytes: int, desc, device) -> T.Optional[torch.Tensor]:
     """split-K scratch of one call, from torch's caching allocator (stream-ordered, CUDA-graph safe): the library itself
     keeps no device state, so calls on different streams never share it"""
@@ -76,9 +72,8 @@ def gemm(
         assert r4.shape == (B2, B1, M, N) and r4.stride(3) == 1
         d.residual, d.ldr, d.sr1, d.sr2 = r4.data_ptr(), r4.stride(2), r4.stride(1), r4.stride(0)
     d.alpha, d.act, d.out_f32 = float(alpha), int(act), int(o4.dtype == torch.float32)
-    with torch.cuda.device(a.device):
-        ws = _workspace(_native.lib().rf_gemm_workspace_bytes(C.byref(d)), d, a.device)     # keeps the scratch alive
-        _native.check(_native.lib().rf_gemm_f16(C.byref(d), _stream(a)))
+    ws = _workspace(_native.lib().rf_gemm_workspace_bytes(C.byref(d)), d, a.device)     # keeps the scratch alive
+    _native.call("rf_gemm_f16", a.device, C.byref(d))
     del ws
     return out
 
@@ -130,9 +125,8 @@ def conv2d(
         assert residual.shape == out.shape and residual.is_contiguous()
         d.residual = _f16(residual, "residual").data_ptr()
     d.out, d.alpha, d.act, d.pad_mode = out.data_ptr(), 1.0, int(act), int(pad_far_edge_only)
-    with torch.cuda.device(x.device):
-        ws = _workspace(_native.lib().rf_conv2d_workspace_bytes(C.byref(d)), d, x.device)
-        _native.check(_native.lib().rf_conv2d_f16(C.byref(d), _stream(x)))
+    ws = _workspace(_native.lib().rf_conv2d_workspace_bytes(C.byref(d)), d, x.device)
+    _native.call("rf_conv2d_f16", x.device, C.byref(d))
     del ws
     return out
 
@@ -171,8 +165,7 @@ def conv2d_upsample2x(x: torch.Tensor, w_phases: torch.Tensor, *, bias: T.Option
     d.x1, d.x2, d.w = x.data_ptr(), None, w_phases.data_ptr()
     d.bias = None if bias is None else _f16(bias, "bias").data_ptr()
     d.out, d.alpha, d.act, d.pad_mode = out.data_ptr(), 1.0, ACT_NONE, 2
-    with torch.cuda.device(x.device):
-        _native.check(_native.lib().rf_conv2d_f16(C.byref(d), _stream(x)))
+    _native.call("rf_conv2d_f16", x.device, C.byref(d))
     return out
 
 
@@ -192,10 +185,8 @@ def group_norm(x: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, groups:
     HW = x.numel() // (B * C1)
     y = torch.empty(x.shape[:-1] + (C,), dtype=torch.float16, device=x.device)
     stats = torch.empty((_native.lib().rf_group_norm_scratch_floats(B, HW, groups),), dtype=torch.float32, device=x.device)
-    with torch.cuda.device(x.device):
-        _native.check(_native.lib().rf_group_norm_cat_f16(
-            x.data_ptr(), None if x2 is None else x2.data_ptr(), C1, B, HW, C, groups, gamma.data_ptr(), beta.data_ptr(),
-            float(eps), int(silu), y.data_ptr(), stats.data_ptr(), _stream(x)))
+    _native.call("rf_group_norm_cat_f16", x.device, x.data_ptr(), None if x2 is None else x2.data_ptr(), C1, B, HW, C,
+                 groups, gamma.data_ptr(), beta.data_ptr(), float(eps), int(silu), y.data_ptr(), stats.data_ptr())
     return y
 
 
@@ -204,9 +195,8 @@ def layer_norm(x: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, eps: fl
     assert x.is_contiguous()
     C = x.shape[-1]
     y = torch.empty_like(x)
-    with torch.cuda.device(x.device):
-        _native.check(_native.lib().rf_layer_norm_f16(x.data_ptr(), x.numel() // C, C, gamma.data_ptr(), beta.data_ptr(),
-                                                      float(eps), y.data_ptr(), _stream(x)))
+    _native.call("rf_layer_norm_f16", x.device, x.data_ptr(), x.numel() // C, C, gamma.data_ptr(), beta.data_ptr(),
+                 float(eps), y.data_ptr())
     return y
 
 
@@ -215,8 +205,7 @@ def geglu(x: torch.Tensor) -> torch.Tensor:
     assert x.is_contiguous()
     inner = x.shape[-1] // 2
     y = torch.empty(x.shape[:-1] + (inner,), dtype=torch.float16, device=x.device)
-    with torch.cuda.device(x.device):
-        _native.check(_native.lib().rf_geglu_f16(x.data_ptr(), x.numel() // (2 * inner), inner, y.data_ptr(), _stream(x)))
+    _native.call("rf_geglu_f16", x.device, x.data_ptr(), x.numel() // (2 * inner), inner, y.data_ptr())
     return y
 
 
@@ -225,8 +214,7 @@ def softmax_rows_(x: torch.Tensor, n: int) -> torch.Tensor:
     _f16(x, "x")
     assert x.is_contiguous()
     pitch = x.shape[-1]
-    with torch.cuda.device(x.device):
-        _native.check(_native.lib().rf_softmax_rows_f16(x.data_ptr(), x.numel() // pitch, n, pitch, x.data_ptr(), _stream(x)))
+    _native.call("rf_softmax_rows_f16", x.device, x.data_ptr(), x.numel() // pitch, n, pitch, x.data_ptr())
     return x
 
 
@@ -234,19 +222,7 @@ def upsample2x(x: torch.Tensor) -> torch.Tensor:
     _f16(x, "x")
     B, H, W, C = x.shape
     y = torch.empty((B, 2 * H, 2 * W, C), dtype=torch.float16, device=x.device)
-    with torch.cuda.device(x.device):
-        _native.check(_native.lib().rf_upsample2x_f16(x.data_ptr(), B, H, W, C, y.data_ptr(), _stream(x)))
-    return y
-
-
-def concat_channels(a: torch.Tensor, b: torch.Tensor) -> torch.Tensor:
-    _f16(a, "a"), _f16(b, "b")
-    assert a.shape[:-1] == b.shape[:-1] and a.is_contiguous() and b.is_contiguous()
-    Ca, Cb = a.shape[-1], b.shape[-1]
-    y = torch.empty(a.shape[:-1] + (Ca + Cb,), dtype=torch.float16, device=a.device)
-    with torch.cuda.device(a.device):
-        _native.check(_native.lib().rf_concat_channels_f16(a.data_ptr(), b.data_ptr(), a.numel() // Ca, Ca, Cb,
-                                                           y.data_ptr(), _stream(a)))
+    _native.call("rf_upsample2x_f16", x.device, x.data_ptr(), B, H, W, C, y.data_ptr())
     return y
 
 
@@ -256,9 +232,8 @@ def conv_in(x_nchw: torch.Tensor, w: torch.Tensor, bias: torch.Tensor) -> torch.
     B, Cin, H, W = x_nchw.shape
     Cout = w.shape[0]
     y = torch.empty((B, H, W, Cout), dtype=torch.float16, device=x_nchw.device)
-    with torch.cuda.device(x_nchw.device):
-        _native.check(_native.lib().rf_conv_in_f16(x_nchw.contiguous().data_ptr(), w.data_ptr(), bias.data_ptr(), B, Cin,
-                                                   H, W, Cout, y.data_ptr(), _stream(x_nchw)))
+    _native.call("rf_conv_in_f16", x_nchw.device, x_nchw.contiguous().data_ptr(), w.data_ptr(), bias.data_ptr(), B, Cin,
+                 H, W, Cout, y.data_ptr())
     return y
 
 
@@ -268,9 +243,8 @@ def conv_out(x_nhwc: torch.Tensor, w_packed: torch.Tensor, bias: torch.Tensor) -
     B, H, W, Cin = x_nhwc.shape
     Cout = w_packed.shape[0]
     y = torch.empty((B, Cout, H, W), dtype=torch.float16, device=x_nhwc.device)
-    with torch.cuda.device(x_nhwc.device):
-        _native.check(_native.lib().rf_conv_out_f16(x_nhwc.data_ptr(), w_packed.data_ptr(), bias.data_ptr(), B, H, W, Cin,
-                                                    Cout, y.data_ptr(), _stream(x_nhwc)))
+    _native.call("rf_conv_out_f16", x_nhwc.device, x_nhwc.data_ptr(), w_packed.data_ptr(), bias.data_ptr(), B, H, W,
+                 Cin, Cout, y.data_ptr())
     return y
 
 
@@ -278,16 +252,14 @@ def timestep_embedding(t: torch.Tensor, dim: int) -> torch.Tensor:
     """t: fp32 (B,) device tensor -> (B, dim) fp16 [cos | sin]."""
     assert t.is_cuda and t.dtype == torch.float32
     out = torch.empty((t.shape[0], dim), dtype=torch.float16, device=t.device)
-    with torch.cuda.device(t.device):
-        _native.check(_native.lib().rf_timestep_embedding_f16(t.data_ptr(), t.shape[0], dim, out.data_ptr(), _stream(t)))
+    _native.call("rf_timestep_embedding_f16", t.device, t.data_ptr(), t.shape[0], dim, out.data_ptr())
     return out
 
 
 def silu(x: torch.Tensor) -> torch.Tensor:
     _f16(x, "x")
     y = torch.empty_like(x)
-    with torch.cuda.device(x.device):
-        _native.check(_native.lib().rf_silu_f16(x.data_ptr(), x.numel(), y.data_ptr(), _stream(x)))
+    _native.call("rf_silu_f16", x.device, x.data_ptr(), x.numel(), y.data_ptr())
     return y
 
 
@@ -301,20 +273,18 @@ def cfg_pndm_step(eps_pair, guidance, hist, coef, sample, ca, cb, want_eps=True)
     prev = torch.empty_like(sample)
     h = [None if i >= len(hist) else hist[i].data_ptr() for i in range(3)]
     c4 = (C.c_float * 4)(*[float(v) for v in coef])
-    with torch.cuda.device(sample.device):
-        _native.check(_native.lib().rf_cfg_pndm_step_f16(
-            eps_pair.data_ptr(), n, float(guidance), h[0], h[1], h[2], c4, sample.data_ptr(), float(ca), float(cb),
-            None if eps_out is None else eps_out.data_ptr(), prev.data_ptr(), _stream(sample)))
+    _native.call("rf_cfg_pndm_step_f16", sample.device, eps_pair.data_ptr(), n, float(guidance), h[0], h[1], h[2], c4,
+                 sample.data_ptr(), float(ca), float(cb), None if eps_out is None else eps_out.data_ptr(),
+                 prev.data_ptr())
     return eps_out, prev
 
 
 def axpby(x, noise, a, b, mask=None, z=None):
     _f16(x, "x")
     y = torch.empty_like(x)
-    with torch.cuda.device(x.device):
-        _native.check(_native.lib().rf_axpby_f16(x.data_ptr(), noise.data_ptr(), float(a), float(b),
-                                                 None if mask is None else mask.data_ptr(),
-                                                 None if z is None else z.data_ptr(), x.numel(), y.data_ptr(), _stream(x)))
+    _native.call("rf_axpby_f16", x.device, x.data_ptr(), noise.data_ptr(), float(a), float(b),
+                 None if mask is None else mask.data_ptr(), None if z is None else z.data_ptr(), x.numel(),
+                 y.data_ptr())
     return y
 
 
@@ -324,9 +294,8 @@ def conv1x1_small(x_nchw: torch.Tensor, w: torch.Tensor, bias: torch.Tensor, in_
     B, Cin, H, W = x_nchw.shape
     Cout = w.shape[0]
     y = torch.empty((B, Cout, H, W), dtype=torch.float16, device=x_nchw.device)
-    with torch.cuda.device(x_nchw.device):
-        _native.check(_native.lib().rf_conv1x1_small_f16(x_nchw.contiguous().data_ptr(), w.data_ptr(), bias.data_ptr(), B, Cin,
-                                                         Cout, H * W, float(in_scale), y.data_ptr(), _stream(x_nchw)))
+    _native.call("rf_conv1x1_small_f16", x_nchw.device, x_nchw.contiguous().data_ptr(), w.data_ptr(), bias.data_ptr(),
+                 B, Cin, Cout, H * W, float(in_scale), y.data_ptr())
     return y
 
 
@@ -338,9 +307,8 @@ def attention(q: torch.Tensor, k: torch.Tensor, vt: torch.Tensor, heads: int, nk
     d = C // heads
     assert q.is_contiguous() and k.is_contiguous() and vt.is_contiguous() and k.shape[1] == nk
     out = torch.empty_like(q)
-    with torch.cuda.device(q.device):
-        _native.check(_native.lib().rf_attention_masked_f16(q.data_ptr(), k.data_ptr(), vt.data_ptr(), out.data_ptr(), B, heads,
-                                                            Nq, nk, d, vt.shape[-1], float(d) ** -0.5, int(causal), _stream(q)))
+    _native.call("rf_attention_masked_f16", q.device, q.data_ptr(), k.data_ptr(), vt.data_ptr(), out.data_ptr(), B,
+                 heads, Nq, nk, d, vt.shape[-1], float(d) ** -0.5, int(causal))
     return out
 
 
@@ -350,8 +318,7 @@ def vae_image_to_u8(x_nchw: torch.Tensor) -> torch.Tensor:
     B, Cc, H, W = x_nchw.shape
     assert Cc == 3
     y = torch.empty((B, H, W, 3), dtype=torch.uint8, device=x_nchw.device)
-    with torch.cuda.device(x_nchw.device):
-        _native.check(_native.lib().rf_vae_image_to_u8(x_nchw.contiguous().data_ptr(), B, H, W, y.data_ptr(), _stream(x_nchw)))
+    _native.call("rf_vae_image_to_u8", x_nchw.device, x_nchw.contiguous().data_ptr(), B, H, W, y.data_ptr())
     return y
 
 
@@ -366,7 +333,6 @@ def slerp(alphas, v0: torch.Tensor, v1: torch.Tensor, dot_threshold: float = 0.9
     al = alphas.to(device=v0.device, dtype=torch.float32).contiguous()
     out = torch.empty_like(v0)
     scratch = torch.empty(3 * B, dtype=torch.float32, device=v0.device)
-    with torch.cuda.device(v0.device):
-        _native.check(_native.lib().rf_slerp_f16(v0.contiguous().data_ptr(), v1.contiguous().data_ptr(), B, n, al.data_ptr(),
-                                                 float(dot_threshold), out.data_ptr(), scratch.data_ptr(), _stream(v0)))
+    _native.call("rf_slerp_f16", v0.device, v0.contiguous().data_ptr(), v1.contiguous().data_ptr(), B, n, al.data_ptr(),
+                 float(dot_threshold), out.data_ptr(), scratch.data_ptr())
     return out

@@ -85,10 +85,8 @@ def spectrogram_from_image_device(
     H, W, C = rgb.shape
     assert C == 3
     out = torch.empty((2 if stereo else 1, H, W), dtype=torch.float32, device=rgb.device)
-    with torch.cuda.device(rgb.device):
-        _native.check(_native.lib().rf_image_to_mel(rgb.data_ptr(), H, W, int(stereo), float(power),
-                                                    float(max_value), out.data_ptr(),
-                                                    _native.stream_ptr(rgb.device)))
+    _native.call("rf_image_to_mel", rgb.device, rgb.data_ptr(), H, W, int(stereo), float(power), float(max_value),
+                 out.data_ptr())
     return out
 
 
@@ -103,7 +101,5 @@ def image_from_spectrogram_device(spectrogram: torch.Tensor, power: float = 0.25
         raise NotImplementedError(f"Unsupported number of channels: {C}")
     img = torch.empty((H, W, 3), dtype=torch.uint8, device=s.device)
     mx = torch.empty((), dtype=torch.float32, device=s.device)
-    with torch.cuda.device(s.device):
-        _native.check(_native.lib().rf_mel_to_image(s.data_ptr(), C, H, W, float(power), img.data_ptr(),
-                                                    mx.data_ptr(), _native.stream_ptr(s.device)))
+    _native.call("rf_mel_to_image", s.device, s.data_ptr(), C, H, W, float(power), img.data_ptr(), mx.data_ptr())
     return img, mx

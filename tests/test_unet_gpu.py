@@ -61,8 +61,6 @@ def test_elementwise_ops_match_torch(native_lib):
     assert (got.float()[..., :77] - ref).abs().max() < 1e-3 and float(got[..., 77:].abs().max()) == 0
     x = torch.randn(2, 4, 6, 64, device="cuda").half()
     assert torch.equal(ops.upsample2x(x), F.interpolate(x.permute(0, 3, 1, 2), scale_factor=2.0, mode="nearest").permute(0, 2, 3, 1))
-    a, bb = torch.randn(2, 3, 3, 128, device="cuda").half(), torch.randn(2, 3, 3, 64, device="cuda").half()
-    assert torch.equal(ops.concat_channels(a, bb), torch.cat([a, bb], dim=-1))
     # edge convolutions: register-blocked kernels (W % 4 == 0, Cout/Cin in {64, 128, 320}) and the generic fallback
     for (B, Cin, H, W, Cout) in ((2, 4, 12, 12, 320), (1, 3, 8, 20, 128), (3, 4, 5, 8, 64), (2, 4, 6, 7, 320),
                                  (1, 4, 9, 12, 96), (2, 4, 8, 8, 512)):
