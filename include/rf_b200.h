@@ -282,6 +282,14 @@ int rf_slerp_f16(const void* v0, const void* v1, int B, long n, const float* d_a
 int rf_cfg_pndm_step_f16(const void* eps_pair, long n, float guidance, const void* h1, const void* h2,
                          const void* h3, const float* coef4, const void* sample, float ca, float cb,
                          void* eps_out, void* prev_sample, void* stream);
+/* classifier-free guidance + DPM-Solver++ (2M, midpoint) update on n = elements of ONE batch half:
+ *   eps = eps_u + g (eps_t - eps_u) (fp16, as rf_cfg_pndm_step_f16); x0 = (x - sigma_s0 eps) / alpha_s0;
+ *   prev = c_x x + c_0 x0 + c_1 (x0 - m1), the last term only when m1 (the previous step's x0) is given.
+ *   The host passes c_x = sigma_t / sigma_s0, c_0 = -alpha_t (e^-h - 1), c_1 = c_0 / (2 r0).  fp32 math with explicit
+ *   roundings; x0_out receives x0 in fp16 (the history of the next step), and prev is computed from that fp16 x0. */
+int rf_cfg_dpmpp_step_f16(const void* eps_pair, long n, float guidance, const void* sample, const void* m1,
+                          float alpha_s0, float sigma_s0, float c_x, float c_0, float c_1, void* x0_out,
+                          void* prev_sample, void* stream);
 /* y = a*x + b*noise (scheduler.add_noise), optionally y = y*mask + z*(1-mask) (riffusion_pipeline.py:421-425) */
 int rf_axpby_f16(const void* x, const void* noise, float a, float b, const void* mask, const void* z, long n,
                  void* y, void* stream);

@@ -719,9 +719,15 @@ static int conv_impl(const rf_conv_desc* d, void* stream, size_t* query) {
     const int extra = (d->ksize == 3 && d->pad_mode == 1) ? 1 : 0;   // one implicit zero row/column at the far edge
     const int Ho = up2 ? d->H : (d->H + 2 * pad + extra - d->ksize) / d->stride + 1;   // up2: the tile grid is the input grid
     const int Wo = up2 ? d->W : (d->W + 2 * pad + extra - d->ksize) / d->stride + 1;
-    // output pixels per tile
-    int bw = Wo >= 128 ? 128 : Wo;
-    while (BM % bw) --bw;  // bw must divide 128
+    // output pixels per tile.  bw is a power of two (it must divide 128): among those from min(8, bw_max) up to bw_max,
+    // the largest power of two <= min(Wo, 128), take the one that pads Wo least, the larger one on a tie.  Powers of two
+    // keep bw = Wo; 96-, 48- and 24-wide levels (768-pixel-wide clips) get exact 32-, 16- and 8-wide tiles instead of
+    // padding a quarter of the columns.
+    int bw_max = Wo >= 128 ? 128 : Wo;
+    while (BM % bw_max) --bw_max;
+    int bw = bw_max;
+    for (int c = bw_max / 2; c >= 8; c /= 2)
+        if ((Wo + c - 1) / c * c < (Wo + bw - 1) / bw * bw) bw = c;
     int bh = BM / bw;
     if (bh > Ho) bh = Ho;
     while ((BM / bw) % bh) --bh;

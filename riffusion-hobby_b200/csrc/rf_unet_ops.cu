@@ -687,6 +687,31 @@ __global__ void k_cfg_pndm_step(const __half* __restrict__ eps_pair, size_t n, f
     }
 }
 
+// eps = eps_u + g (eps_t - eps_u)               fp16 arithmetic, bit-identical to k_cfg_pndm_step's
+// x0  = (x - sigma_s0 eps) / alpha_s0           DPMSolverMultistepScheduler.convert_model_output ("dpmsolver++")
+// x'  = c_x x + c_0 x0 + c_1 (x0 - m1)          first order (m1 == NULL) or the 2M midpoint update
+// x0 is rounded to fp16 once; x' is computed from that rounded x0, the value the next step reads back as m1.  Every
+// product and sum has an explicit rounding, so the result does not depend on how the compiler contracts.
+__global__ void k_cfg_dpmpp_step(const __half* __restrict__ eps_pair, size_t n, float guidance,
+                                 const __half* __restrict__ sample, const __half* __restrict__ m1, float alpha_s0,
+                                 float sigma_s0, float c_x, float c_0, float c_1, __half* __restrict__ x0_out,
+                                 __half* __restrict__ prev_sample) {
+    for (size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < n;
+         i += static_cast<size_t>(gridDim.x) * blockDim.x) {
+        const __half eu = eps_pair[i], et = eps_pair[n + i];
+        const __half d = __hsub(et, eu);
+        const __half gd = __float2half_rn(__half2float(d) * guidance);
+        const float e = __half2float(__hadd(eu, gd));
+        const float x = __half2float(sample[i]);
+        const __half x0h = __float2half_rn(__fdiv_rn(__fmaf_rn(-sigma_s0, e, x), alpha_s0));
+        x0_out[i] = x0h;
+        const float x0 = __half2float(x0h);
+        float acc = __fmaf_rn(c_0, x0, __fmul_rn(c_x, x));
+        if (m1) acc = __fmaf_rn(c_1, __fsub_rn(x0, __half2float(m1[i])), acc);
+        prev_sample[i] = __float2half_rn(acc);
+    }
+}
+
 // add_noise / mask blend: y = a*x + b*n (scheduler.add_noise), optionally blended y*m + z*(1-m)
 __global__ void k_axpby(const __half* __restrict__ x, const __half* __restrict__ nz, float a, float b,
                         const __half* __restrict__ mask, const __half* __restrict__ z, size_t n,
@@ -1031,6 +1056,19 @@ extern "C" int rf_cfg_pndm_step_f16(const void* eps_pair, long n, float guidance
         static_cast<const __half*>(h2), static_cast<const __half*>(h3), coef4[0], coef4[1], coef4[2], coef4[3],
         static_cast<const __half*>(sample), ca, cb, static_cast<__half*>(eps_out), static_cast<__half*>(prev_sample));
     RF_CUDA_LAUNCH_CHECK("k_cfg_pndm_step");
+    return RF_OK;
+}
+
+extern "C" int rf_cfg_dpmpp_step_f16(const void* eps_pair, long n, float guidance, const void* sample, const void* m1,
+                                     float alpha_s0, float sigma_s0, float c_x, float c_0, float c_1, void* x0_out,
+                                     void* prev_sample, void* stream) {
+    if (!eps_pair || !sample || !x0_out || !prev_sample || n <= 0 || !(alpha_s0 > 0.f))
+        return rf_fail(RF_ERR_INVALID, "rf_cfg_dpmpp_step_f16: bad argument");
+    k_cfg_dpmpp_step<<<grid_for(static_cast<size_t>(n), 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+        static_cast<const __half*>(eps_pair), static_cast<size_t>(n), guidance, static_cast<const __half*>(sample),
+        static_cast<const __half*>(m1), alpha_s0, sigma_s0, c_x, c_0, c_1, static_cast<__half*>(x0_out),
+        static_cast<__half*>(prev_sample));
+    RF_CUDA_LAUNCH_CHECK("k_cfg_dpmpp_step");
     return RF_OK;
 }
 

@@ -119,6 +119,8 @@ SIGNATURES = {
     "rf_cfg_pndm_step_f16": (C.c_int, [C.c_void_p, C.c_long, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p,
                                        C.c_void_p, C.c_void_p, C.c_float, C.c_float, C.c_void_p, C.c_void_p,
                                        C.c_void_p]),
+    "rf_cfg_dpmpp_step_f16": (C.c_int, [C.c_void_p, C.c_long, C.c_float, C.c_void_p, C.c_void_p, C.c_float, C.c_float,
+                                        C.c_float, C.c_float, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p]),
     "rf_axpby_f16": (C.c_int, [C.c_void_p, C.c_void_p, C.c_float, C.c_float, C.c_void_p, C.c_void_p, C.c_long,
                                C.c_void_p, C.c_void_p]),
     "rf_attention_masked_f16": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int,

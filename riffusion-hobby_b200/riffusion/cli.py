@@ -1,5 +1,6 @@
 """Command line front end: the six commands of the reference's `python -m riffusion.cli` (riffusion/cli.py:21-278) with
-the same names, flags and defaults:
+the same names, flags and defaults (`COMMANDS`, what `build_parser()` builds by default), plus this package's
+`text-to-audio`, the app's text-to-audio task as a command (`EXTRA_COMMANDS`; `main` offers both sets):
 
     python -m riffusion.cli audio-to-image --audio clip.wav --image clip.png [--stereo] [--device cuda]
     python -m riffusion.cli image-to-audio --image clip.png --audio clip.wav
@@ -7,6 +8,13 @@ the same names, flags and defaults:
     python -m riffusion.cli sample-clips --audio song.wav --output-dir clips --num-clips 4
     python -m riffusion.cli audio-to-images-batch --audio-dir clips --output-dir images
     python -m riffusion.cli sample-clips-batch --audio-dir songs --output-dir clips
+    python -m riffusion.cli text-to-audio --prompt "jazz with piano" --audio out.wav [--image out.png]
+        [--negative-prompt ...] [--seed 42] [--num-clips 1] [--num-inference-steps 30] [--guidance 7.0] [--width 512]
+        [--scheduler DPMSolverMultistepScheduler] [--use-20k] [--checkpoint DIR] [--device cuda]
+
+`text-to-audio` loads a local diffusers-layout checkpoint directory; with `--num-clips N` > 1 clip i (seed + i) is
+written to out_<seed + i>.wav / .png.  The image carries the spectrogram parameters in its EXIF block, so
+`image-to-audio` turns it back into the same audio.
 
 Each command is a keyword-only function (callable from Python exactly like the reference's); `argh`, which the reference
 uses to turn those functions into sub-commands, is not installed on the GPU image, so `build_parser` derives an
@@ -171,7 +179,46 @@ def sample_clips_batch(*, audio_dir: str, output_dir: str, num_clips_per_file: i
     _run_pool(cut_one, sources, num_threads)
 
 
+def text_to_audio(*, prompt: str, audio: str, image: str = "", negative_prompt: str = "", seed: int = 42,
+                  num_clips: int = 1, num_inference_steps: int = 30, guidance: float = 7.0, width: int = 512,
+                  scheduler: str = "DPMSolverMultistepScheduler", use_20k: bool = False,
+                  checkpoint: str = "riffusion/riffusion-model-v1", device: str = "cuda"):
+    """Generate audio from a text prompt (Stable Diffusion txt2img, then spectrogram image -> audio)."""
+    from riffusion.riffusion_pipeline import RiffusionPipeline
+    from riffusion.util import audio_util
+
+    if use_20k:         # the app's "Use 20kHz" switch
+        params = SpectrogramParams(min_frequency=10, max_frequency=20000, stereo=True)
+    else:
+        params = SpectrogramParams(min_frequency=0, max_frequency=10000, stereo=False)
+    pipe = RiffusionPipeline.load_checkpoint(checkpoint=checkpoint, device=device)
+    out = pipe.text_to_audio(prompt, params=params, negative_prompt=negative_prompt or None, seed=seed,
+                             num_clips=num_clips, num_inference_steps=num_inference_steps, guidance_scale=guidance,
+                             width=width, scheduler=scheduler)
+    images, waves = out["images"].cpu().numpy(), out["waveform"].cpu().numpy()
+
+    def target(path: str, i: int) -> Path:
+        p = Path(path)
+        return p if num_clips == 1 else p.with_name(f"{p.stem}_{seed + i}{p.suffix}")
+
+    for i in range(num_clips):
+        segment = audio_util.apply_filters(
+            audio_util.audio_from_waveform(samples=waves[i], sample_rate=params.sample_rate, normalize=True),
+            compression=False)
+        wav_path = target(audio, i)
+        segment.export(str(wav_path), format=wav_path.suffix[1:])
+        print(f"Wrote {wav_path} ({segment.duration_seconds:.2f} seconds)")
+        if image:
+            picture = Image.fromarray(images[i])
+            picture.getexif().update(params.to_exif().items())
+            img_path = target(image, i)
+            _store_image(picture, img_path, _PIL_FORMAT.get(img_path.suffix[1:].lower(), "PNG"))
+            print(f"Wrote {img_path}")
+
+
 COMMANDS = [audio_to_image, image_to_audio, sample_clips, print_exif, audio_to_images_batch, sample_clips_batch]
+# commands of this package that the reference's CLI does not have; `main` offers them next to COMMANDS
+EXTRA_COMMANDS = [text_to_audio]
 
 
 # ------------------------------------------------------------------------------------------------ argparse front end
@@ -183,11 +230,12 @@ def _str2bool(v: str) -> bool:
     raise argparse.ArgumentTypeError(f"expected a boolean, got {v!r}")
 
 
-def build_parser() -> argparse.ArgumentParser:
-    """argh-style front end: one sub-command per function (underscores -> dashes), one --flag per keyword-only arg."""
+def build_parser(commands: T.Sequence[T.Callable] = tuple(COMMANDS)) -> argparse.ArgumentParser:
+    """argh-style front end: one sub-command per function (underscores -> dashes), one --flag per keyword-only arg.
+    By default the reference's six commands exactly; `main` passes COMMANDS + EXTRA_COMMANDS."""
     parser = argparse.ArgumentParser(prog="riffusion.cli", description=__doc__)
     sub = parser.add_subparsers(dest="command", required=True)
-    for fn in COMMANDS:
+    for fn in commands:
         sp = sub.add_parser(fn.__name__.replace("_", "-"), help=(fn.__doc__ or "").strip())
         sp.set_defaults(_fn=fn)
         for name, prm in inspect.signature(fn).parameters.items():
@@ -204,7 +252,7 @@ def build_parser() -> argparse.ArgumentParser:
 
 
 def main(argv: T.Optional[T.Sequence[str]] = None) -> None:
-    args = vars(build_parser().parse_args(argv))
+    args = vars(build_parser(COMMANDS + EXTRA_COMMANDS).parse_args(argv))
     fn = args.pop("_fn")
     args.pop("command")
     fn(**args)

@@ -25,7 +25,7 @@ from PIL import Image
 
 from riffusion import tc_ops as ops
 from riffusion.datatypes import InferenceInput
-from riffusion.scheduler_b200 import PNDMSchedulerB200
+from riffusion.scheduler_b200 import PNDMSchedulerB200, make_scheduler
 from riffusion.unet_b200 import UNetB200
 from riffusion.util import torch_util
 from riffusion.vae_b200 import VaeB200
@@ -268,18 +268,7 @@ class RiffusionPipeline:
         t_start = max(num_inference_steps - init_timestep + offset, 0)                             # :392
         timesteps = self.scheduler.timesteps[t_start:]
         ctx_cache: T.Dict[str, T.Any] = {}
-        graphed = None
-        if self.use_cuda_graph and do_cfg:
-            from riffusion.graphed import GraphedUNet
-
-            # one captured graph per (latent shape, context shape); a new request only refreshes the cross-attention
-            # K / V^T that the graph reads (capture costs two eager evaluations + instantiation)
-            gkey = (tuple(latents.shape), tuple(context.shape))
-            graphed = self._graphs.get(gkey)
-            if graphed is None:
-                graphed = self._graphs[gkey] = GraphedUNet(self.unet, latents.shape, context)
-            else:
-                graphed.set_context(context)
+        graphed = self._graphed_unet(latents.shape, context) if do_cfg else None
         n_evals = 0
         for t in timesteps:                                                                        # :398
             t_int = int(t)
@@ -313,6 +302,141 @@ class RiffusionPipeline:
             out["images"] = (image / 2 + 0.5).clamp(0, 1).cpu().permute(0, 2, 3, 1).numpy()         # float16 array, like the reference
         return out
 
+    def _graphed_unet(self, latent_shape, context: torch.Tensor):
+        """The CUDA-graph CFG evaluation for this (latent shape, context shape), or None when graphs are off."""
+        if not self.use_cuda_graph:
+            return None
+        from riffusion.graphed import GraphedUNet
+
+        # one captured graph per (latent shape, context shape); a new request only refreshes the cross-attention
+        # K / V^T that the graph reads (capture costs two eager evaluations + instantiation)
+        gkey = (tuple(latent_shape), tuple(context.shape))
+        graphed = self._graphs.get(gkey)
+        if graphed is None:
+            graphed = self._graphs[gkey] = GraphedUNet(self.unet, latent_shape, context)
+        else:
+            graphed.set_context(context)
+        return graphed
+
+    # ------------------------------------------------------------------------------ text -> image
+    @torch.no_grad()
+    def txt2img(self, prompt: str, *, negative_prompt: T.Optional[str] = None, seed: int = 42, num_clips: int = 1,
+                num_inference_steps: int = 30, guidance_scale: float = 7.0, width: int = 512, height: int = 512,
+                scheduler: str = "DPMSolverMultistepScheduler", output_type: T.Optional[str] = "pil",
+                text_embeddings: T.Optional[torch.Tensor] = None, uncond_embeddings: T.Optional[torch.Tensor] = None,
+                latents: T.Optional[torch.Tensor] = None) -> T.Dict[str, T.Any]:
+        """Text to spectrogram image: Stable Diffusion txt2img, the reference app's text-to-audio generation.
+
+        Clip i starts from `torch.randn((1, 4, height/8, width/8))` drawn from a CUDA generator seeded with `seed + i`
+        (one pipeline call per seed in the app); all clips run as one CFG batch.  The prompt and the negative prompt
+        (default "") are encoded without prompt weighting.  `scheduler` is "DPMSolverMultistepScheduler" or
+        "PNDMScheduler"; a fresh instance is used per call.  `width` and `height` must be multiples of 64 (diffusers
+        accepts multiples of 8).  `text_embeddings` / `uncond_embeddings` / `latents` replace the text encoder and the
+        generator draws.  Returns dict(images, latents (1/0.18215-scaled), latents_unscaled, n_unet_evals)."""
+        if width <= 0 or height <= 0 or width % 64 or height % 64:
+            raise ValueError(f"width and height must be positive multiples of 64, got {width}x{height}")
+        if num_clips < 1:
+            raise ValueError("num_clips must be at least 1")
+        sched = make_scheduler(scheduler)
+        sched.set_timesteps(num_inference_steps)
+        dev = self._device
+        do_cfg = guidance_scale > 1.0
+        text = self.embed_text(prompt) if text_embeddings is None else text_embeddings
+        text = text.to(device=dev, dtype=torch.float16)
+        text = text.expand(num_clips, -1, -1) if text.shape[0] == 1 else text
+        if text.shape[0] != num_clips:
+            raise ValueError(f"text_embeddings hold {text.shape[0]} rows for {num_clips} clips")
+        if do_cfg:
+            uncond = self.embed_text(negative_prompt or "") if uncond_embeddings is None else uncond_embeddings
+            uncond = uncond.to(device=dev, dtype=torch.float16)
+            uncond = uncond.expand(num_clips, -1, -1) if uncond.shape[0] == 1 else uncond
+            context = torch.cat([uncond, text]).contiguous()
+        else:
+            context = text.contiguous()
+        shape = (1, 4, height // 8, width // 8)
+        if latents is None:
+            latents = torch.cat([torch.randn(shape, generator=torch.Generator(device=self.device).manual_seed(seed + i),
+                                             device=self.device, dtype=torch.float16) for i in range(num_clips)])
+        latents = latents.to(device=dev, dtype=torch.float16).contiguous()
+        if tuple(latents.shape) != (num_clips,) + shape[1:]:
+            raise ValueError(f"latents must be {(num_clips,) + shape[1:]}, got {tuple(latents.shape)}")
+        if sched.init_noise_sigma != 1.0:
+            latents = (latents * sched.init_noise_sigma).contiguous()
+
+        ctx_cache: T.Dict[str, T.Any] = {}
+        graphed = self._graphed_unet(latents.shape, context) if do_cfg else None
+        n_evals = 0
+        for t in sched.timesteps:
+            t_int = int(t)
+            if graphed is not None:
+                eps_pair = graphed(latents, t_int)
+            else:
+                model_in = torch.cat([latents] * 2) if do_cfg else latents
+                eps_pair = self.unet(model_in, t_int, encoder_hidden_states=context, ctx_cache=ctx_cache).sample
+            n_evals += 1
+            if not do_cfg:
+                eps_pair = torch.cat([eps_pair, eps_pair])
+            latents = sched.step_cfg(eps_pair, guidance_scale if do_cfg else 0.0, t_int, latents)
+
+        scaled = (1.0 / VAE_SCALE) * latents
+        out: T.Dict[str, T.Any] = dict(latents=scaled, latents_unscaled=latents, n_unet_evals=n_evals)
+        if output_type == "latent" or self.vae is None:
+            out["images"] = None
+            return out
+        image = self.vae.decode(scaled).sample
+        if output_type == "pil":
+            out["images"] = [Image.fromarray(im) for im in ops.vae_image_to_u8(image).cpu().numpy()]
+        else:
+            out["images"] = (image / 2 + 0.5).clamp(0, 1).cpu().permute(0, 2, 3, 1).numpy()
+        return out
+
+    @torch.no_grad()
+    def text_to_audio(self, prompt: str, *, params=None, negative_prompt: T.Optional[str] = None, seed: int = 42,
+                      num_clips: int = 1, num_inference_steps: int = 30, guidance_scale: float = 7.0, width: int = 512,
+                      height: T.Optional[int] = None, scheduler: str = "DPMSolverMultistepScheduler",
+                      text_embeddings: T.Optional[torch.Tensor] = None, uncond_embeddings: T.Optional[torch.Tensor] = None,
+                      latents: T.Optional[torch.Tensor] = None, converter=None,
+                      init_angles: T.Optional[torch.Tensor] = None) -> T.Dict[str, torch.Tensor]:
+        """Text to audio on the device: `txt2img` with height = params.num_frequencies, then VAE decode -> uint8 image ->
+        mel amplitudes (`audio_from_spectrogram_image` semantics: R plane for mono, G and B for stereo, max_value 30e6)
+        -> inverse mel + Griffin-Lim.  `params` defaults to mono 0-10 kHz.  Returns device tensors: images (B, H, W, 3)
+        uint8, waveform (B, channels, hop * (W - 1)) fp32 before peak normalisation, latents, latents_unscaled,
+        n_unet_evals."""
+        from riffusion.spectrogram_converter import SpectrogramConverter
+        from riffusion.spectrogram_params import SpectrogramParams
+
+        if params is None:
+            params = SpectrogramParams(min_frequency=0, max_frequency=10000, stereo=False)
+        if height is not None and height != params.num_frequencies:
+            raise ValueError(f"height {height} differs from params.num_frequencies {params.num_frequencies}")
+        if converter is None:
+            converter = SpectrogramConverter(params, device=self.device)
+        if converter.p != params:
+            raise ValueError("converter was built for other SpectrogramParams")
+        out = self.txt2img(prompt, negative_prompt=negative_prompt, seed=seed, num_clips=num_clips,
+                           num_inference_steps=num_inference_steps, guidance_scale=guidance_scale, width=width,
+                           height=params.num_frequencies, scheduler=scheduler, output_type="latent",
+                           text_embeddings=text_embeddings, uncond_embeddings=uncond_embeddings, latents=latents)
+        u8, wave = self._latents_to_audio(out["latents"], converter, params.stereo, init_angles)
+        return dict(images=u8, waveform=wave, latents=out["latents"], latents_unscaled=out["latents_unscaled"],
+                    n_unet_evals=out["n_unet_evals"])
+
+    def _latents_to_audio(self, scaled_latents: torch.Tensor, converter, stereo: bool,
+                          init_angles: T.Optional[torch.Tensor]) -> T.Tuple[torch.Tensor, torch.Tensor]:
+        """VAE decode -> uint8 image (B, H, W, 3) -> mel amplitudes (B, channels, H, W) -> waveform (B, channels, L),
+        without leaving the device."""
+        from riffusion import _native
+
+        image = self.vae.decode(scaled_latents).sample
+        u8 = ops.vae_image_to_u8(image)
+        B, H, W, _ = u8.shape
+        mel = torch.empty((B, 2 if stereo else 1, H, W), dtype=torch.float32, device=u8.device)
+        p = converter.p
+        for i in range(B):
+            _native.call("rf_image_to_mel", u8.device, u8[i].data_ptr(), H, W, int(stereo), float(p.power_for_image),
+                         30e6, mel[i].data_ptr())
+        return u8, converter.waveform_from_mel_amplitudes(mel, init_angles)
+
     # ------------------------------------------------------------------------------ batched request -> audio
     @torch.no_grad()
     def generate_clips(self, text_embeddings: torch.Tensor, uncond_embeddings: torch.Tensor, init_latents: torch.Tensor,
@@ -323,23 +447,12 @@ class RiffusionPipeline:
         This is what `server.compute_request` does per request (riffuse, then audio_from_spectrogram_image,
         server.py:145-164) without leaving the GPU in between.  Returns device tensors:
         images (B,512,512,3) uint8, waveform (B, L) fp32, latents."""
-        from riffusion import _native
-
         out = self.interpolate_img2img(
             text_embeddings=text_embeddings, init_latents=init_latents, generator_a=None, generator_b=None,
             interpolate_alpha=0.0, strength_a=strength, strength_b=strength, num_inference_steps=num_inference_steps,
             guidance_scale=guidance_scale, uncond_embeddings=uncond_embeddings, noise=noise, output_type="latent")
-        latents = out["latents_unscaled"]
-        image = self.vae.decode(out["latents"]).sample
-        u8 = ops.vae_image_to_u8(image)
-        B, H, W, _ = u8.shape
-        mel = torch.empty((B, H, W), dtype=torch.float32, device=u8.device)
-        p = converter.p
-        for i in range(B):
-            _native.call("rf_image_to_mel", u8.device, u8[i].data_ptr(), H, W, 0, float(p.power_for_image), 30e6,
-                         mel[i].data_ptr())
-        wave = converter.waveform_from_mel_amplitudes(mel, init_angles)
-        return dict(images=u8, waveform=wave, latents=out["latents"], latents_unscaled=latents,
+        u8, wave = self._latents_to_audio(out["latents"], converter, False, init_angles)
+        return dict(images=u8, waveform=wave[:, 0], latents=out["latents"], latents_unscaled=out["latents_unscaled"],
                     n_unet_evals=out["n_unet_evals"])
 
     @staticmethod

@@ -279,6 +279,23 @@ def cfg_pndm_step(eps_pair, guidance, hist, coef, sample, ca, cb, want_eps=True)
     return eps_out, prev
 
 
+def cfg_dpmpp_step(eps_pair, guidance, sample, m1, coefs):
+    """Guidance combine + one DPM-Solver++ update.  eps_pair: (2B, ...) fp16 [uncond | text]; m1: the previous step's x0
+    (second order) or None (first order); coefs = (alpha_s0, sigma_s0, c_x, c_0, c_1).  Returns (x0, prev_sample)."""
+    _f16(eps_pair, "eps_pair"), _f16(sample, "sample")
+    n = sample.numel()
+    assert eps_pair.numel() == 2 * n and eps_pair.is_contiguous() and sample.is_contiguous()
+    if m1 is not None:
+        _f16(m1, "m1")
+        assert m1.shape == sample.shape and m1.is_contiguous()
+    alpha_s0, sigma_s0, c_x, c_0, c_1 = (float(v) for v in coefs)
+    x0 = torch.empty_like(sample)
+    prev = torch.empty_like(sample)
+    _native.call("rf_cfg_dpmpp_step_f16", sample.device, eps_pair.data_ptr(), n, float(guidance), sample.data_ptr(),
+                 _native.ptr(m1), alpha_s0, sigma_s0, c_x, c_0, c_1, x0.data_ptr(), prev.data_ptr())
+    return x0, prev
+
+
 def axpby(x, noise, a, b, mask=None, z=None):
     _f16(x, "x")
     y = torch.empty_like(x)
