@@ -159,6 +159,21 @@ int rf_mel_to_image(const float* d_mel, int channels, int height, int width, flo
  * d_wave f32[C][L] -> d_pcm i16[L][C]; x *= 32767/max|x| over all channels, truncate. */
 int rf_wave_to_int16(const float* d_wave, int channels, int L, int normalize, int16_t* d_pcm,
                      float* d_scratch, void* stream);
+/* PIL Image.resize((out_w, out_h), Image.BICUBIC) on a batch of uint8 images, bit-exact with Pillow (libImaging/Resample.c):
+ * fp64 tap tables rounded to int32 with 22 fractional bits on the host, integer multiply-adds on the device, horizontal
+ * pass first, 8-bit storage between the passes.  The audio-to-audio task resizes each clip's spectrogram image to a
+ * 32-pixel stride and back (riffusion/streamlit/tasks/audio_to_audio.py:286-287,419-425).
+ *   d_in  u8[B][in_h][in_w][channels], channels 1..4;  d_out u8[B][out_h][out_w][channels]
+ *   d_out_f16 (optional, NULL = none): fp16 [B][channels][out_h][out_w] = 2 * (u8 / 255) - 1 in fp32, the VAE input
+ *             (riffusion_pipeline.preprocess_image arithmetic)
+ *   d_workspace: rf_resize_bicubic_workspace_bytes(...) bytes (tap tables + the intermediate image). */
+size_t rf_resize_bicubic_workspace_bytes(int B, int in_h, int in_w, int channels, int out_h, int out_w);
+int rf_resize_bicubic_u8(const uint8_t* d_in, int B, int in_h, int in_w, int channels, int out_h, int out_w,
+                         uint8_t* d_out, void* d_out_f16, void* d_workspace, size_t workspace_bytes, void* stream);
+/* Host only: the taps per output of an in_size -> out_size resize (-1 on a bad size), and the table the device passes use,
+ * int32[out_size][2 + taps] = (first input index, taps used, taps...); `bytes` must equal its size. */
+int rf_resize_bicubic_taps(int in_size, int out_size);
+int rf_resize_bicubic_table(int in_size, int out_size, int32_t* dst, size_t bytes);
 
 
 /* ==== path (b): tensor-core building blocks (wgmma / TMA) ==================================

@@ -132,6 +132,11 @@ SIGNATURES = {
     "rf_mel_to_image": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_float, C.c_void_p, C.c_void_p,
                                   C.c_void_p]),
     "rf_wave_to_int16": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "rf_resize_bicubic_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]),
+    "rf_resize_bicubic_u8": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p,
+                                       C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "rf_resize_bicubic_taps": (C.c_int, [C.c_int, C.c_int]),
+    "rf_resize_bicubic_table": (C.c_int, [C.c_int, C.c_int, C.c_void_p, C.c_size_t]),
 }
 
 _lib = None

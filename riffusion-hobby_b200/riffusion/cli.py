@@ -11,6 +11,11 @@ the same names, flags and defaults (`COMMANDS`, what `build_parser()` builds by 
     python -m riffusion.cli text-to-audio --prompt "jazz with piano" --audio out.wav [--image out.png]
         [--negative-prompt ...] [--seed 42] [--num-clips 1] [--num-inference-steps 30] [--guidance 7.0] [--width 512]
         [--scheduler DPMSolverMultistepScheduler] [--use-20k] [--checkpoint DIR] [--device cuda]
+    python -m riffusion.cli audio-to-audio --audio song.wav --output riffed.wav --prompt "jazz with piano"
+        [--image-dir clips] [--negative-prompt ...] [--seed 42] [--denoising 0.55] [--num-inference-steps 25]
+        [--guidance 7.0] [--scheduler DPMSolverMultistepScheduler] [--start-time-s 0] [--duration-s 20]
+        [--clip-duration-s 5] [--overlap-duration-s 0.2] [--prompt-b ... [--seed-b N] [--denoising-b X]]
+        [--max-batch 32] [--use-20k] [--checkpoint DIR] [--device cuda]
 
 `text-to-audio` loads a local diffusers-layout checkpoint directory; with `--num-clips N` > 1 clip i (seed + i) is
 written to out_<seed + i>.wav / .png.  The image carries the spectrogram parameters in its EXIF block, so
@@ -216,9 +221,48 @@ def text_to_audio(*, prompt: str, audio: str, image: str = "", negative_prompt: 
             print(f"Wrote {img_path}")
 
 
+def audio_to_audio(*, audio: str, output: str, prompt: str, image_dir: str = "", negative_prompt: str = "",
+                   seed: int = 42, denoising: float = 0.55, num_inference_steps: int = 25, guidance: float = 7.0,
+                   scheduler: str = "DPMSolverMultistepScheduler", start_time_s: float = 0.0, duration_s: float = 20.0,
+                   clip_duration_s: float = 5.0, overlap_duration_s: float = 0.2, prompt_b: str = "", seed_b: int = -1,
+                   denoising_b: float = -1.0, max_batch: int = 32, use_20k: bool = False,
+                   checkpoint: str = "riffusion/riffusion-model-v1", device: str = "cuda"):
+    """Riff a track with a text prompt (overlapping clips, img2img, crossfaded back together); with --prompt-b,
+    interpolate from --prompt to --prompt-b along the track (--seed-b / --denoising-b: -1 = same as the first end)."""
+    from riffusion.riffusion_pipeline import RiffusionPipeline
+
+    if use_20k:         # the app's "Use 20kHz" switch
+        params = SpectrogramParams(min_frequency=10, max_frequency=20000, stereo=True)
+    else:
+        params = SpectrogramParams(min_frequency=0, max_frequency=10000, stereo=False)
+    track = AudioSegment.from_file(audio)
+    pipe = RiffusionPipeline.load_checkpoint(checkpoint=checkpoint, device=device)
+    out = pipe.audio_to_audio(
+        track, prompt, params=params, start_time_s=start_time_s, duration_s=duration_s, clip_duration_s=clip_duration_s,
+        overlap_duration_s=overlap_duration_s, negative_prompt=negative_prompt or None, seed=seed, denoising=denoising,
+        num_inference_steps=num_inference_steps, guidance_scale=guidance, scheduler=scheduler,
+        prompt_b=prompt_b or None, seed_b=None if seed_b < 0 else seed_b,
+        denoising_b=None if denoising_b < 0 else denoising_b, max_batch=max_batch)
+    segment = out["segment"]
+    segment.export(output, format=Path(output).suffix[1:])
+    print(f"Wrote {output} ({segment.duration_seconds:.2f} seconds, {len(out['clip_start_times'])} clips)")
+    if image_dir:
+        target = Path(image_dir)
+        target.mkdir(parents=True, exist_ok=True)
+        for kind in ("source", "riffed"):
+            images = out["source_images" if kind == "source" else "images"].cpu().numpy()
+            for i, im in enumerate(images):
+                picture = Image.fromarray(im)
+                picture.getexif().update(params.to_exif().items())
+                _store_image(picture, target / f"clip_{i}_{kind}.png", "PNG")
+        print(f"Wrote {2 * len(images)} images to {image_dir}")
+
+
 COMMANDS = [audio_to_image, image_to_audio, sample_clips, print_exif, audio_to_images_batch, sample_clips_batch]
 # commands of this package that the reference's CLI does not have; `main` offers them next to COMMANDS
 EXTRA_COMMANDS = [text_to_audio]
+# the track-level command, offered by `main` after EXTRA_COMMANDS
+TRACK_COMMANDS = [audio_to_audio]
 
 
 # ------------------------------------------------------------------------------------------------ argparse front end
@@ -252,7 +296,7 @@ def build_parser(commands: T.Sequence[T.Callable] = tuple(COMMANDS)) -> argparse
 
 
 def main(argv: T.Optional[T.Sequence[str]] = None) -> None:
-    args = vars(build_parser(COMMANDS + EXTRA_COMMANDS).parse_args(argv))
+    args = vars(build_parser(COMMANDS + EXTRA_COMMANDS + TRACK_COMMANDS).parse_args(argv))
     fn = args.pop("_fn")
     args.pop("command")
     fn(**args)

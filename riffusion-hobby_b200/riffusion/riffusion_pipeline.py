@@ -139,16 +139,27 @@ class RiffusionPipeline:
         return outputs["images"][0]
 
     @torch.no_grad()
-    def riffuse_batch(self, inputs: T.Sequence[InferenceInput], init_images: T.Union[Image.Image, T.Sequence[Image.Image]],
-                      mask_image: T.Optional[Image.Image] = None, use_reweighting: bool = True) -> T.List[Image.Image]:
+    def riffuse_batch(self, inputs: T.Sequence[InferenceInput],
+                      init_images: T.Union[None, Image.Image, T.Sequence[Image.Image]],
+                      mask_image: T.Optional[Image.Image] = None, use_reweighting: bool = True, *,
+                      moments: T.Optional[T.Tuple[torch.Tensor, torch.Tensor]] = None,
+                      output_type: str = "pil") -> T.List[T.Any]:
         """`riffuse` for a list of requests in one batched denoising loop (SURVEY 8(f)-2) — what
         streamlit/tasks/interpolation.py:146-164 does one request at a time.  Every request draws exactly what `riffuse`
         draws for it (posterior noise and noise_a from generator(start.seed), noise_b from generator(end.seed), per-request
         alpha for the slerp and the prompt interpolation), so result i equals `riffuse(inputs[i], ...)` up to the batch-size
         dependent accumulation order of the kernels.  Requests are grouped by (strength, guidance, steps): the PNDM state
-        and the guidance scalar are shared inside a group."""
-        images = [init_images] * len(inputs) if isinstance(init_images, Image.Image) else list(init_images)
-        assert len(images) == len(inputs)
+        and the guidance scalar are shared inside a group.
+
+        `moments` = (mean, logvar), each (len(inputs), 4, h, w), replaces the VAE encoding of `init_images` (pass None
+        for them): request i starts from row i.  `output_type="latent"` returns each request's (1, 4, h, w) latents
+        (1/0.18215-scaled) instead of a PIL image."""
+        if moments is None:
+            images = [init_images] * len(inputs) if isinstance(init_images, Image.Image) else list(init_images)
+            assert len(images) == len(inputs)
+        else:
+            assert init_images is None and moments[0].shape[0] == len(inputs)
+        from riffusion.vae_b200 import _Posterior
         embed = self.embed_text_weighted if use_reweighting else self.embed_text
         groups: T.Dict[T.Tuple, T.List[int]] = {}
         for i, inp in enumerate(inputs):
@@ -169,7 +180,12 @@ class RiffusionPipeline:
                 inp = inputs[i]
                 e0, e1 = embed(inp.start.prompt), embed(inp.end.prompt)
                 texts.append(e0 + inp.alpha * (e1 - e0))
-                lats.append(self.encode_image(images[i], torch.Generator(device=self.device).manual_seed(inp.start.seed)))
+                g_post = torch.Generator(device=self.device).manual_seed(inp.start.seed)
+                if moments is None:
+                    lats.append(self.encode_image(images[i], g_post))
+                else:
+                    post = _Posterior(moments[0][i:i + 1], moments[1][i:i + 1])
+                    lats.append(VAE_SCALE * post.sample(generator=g_post))
                 ga = torch.Generator(device=self.device).manual_seed(inp.start.seed)
                 gb = torch.Generator(device=self.device).manual_seed(inp.end.seed)
                 shape = lats[-1].shape
@@ -184,9 +200,9 @@ class RiffusionPipeline:
             out = self.interpolate_img2img(
                 text_embeddings=torch.cat(texts), init_latents=torch.cat(lats), mask=mask, generator_a=None, generator_b=None,
                 interpolate_alpha=0.0, strength_a=strength, strength_b=strength, num_inference_steps=steps,
-                guidance_scale=guidance, noise=noise)
+                guidance_scale=guidance, noise=noise, output_type=output_type)
             for j, i in enumerate(idx):
-                results[i] = out["images"][j]
+                results[i] = out["latents"][j:j + 1] if output_type == "latent" else out["images"][j]
         return results  # type: ignore[return-value]
 
     def encode_image(self, init_image: Image.Image, generator: torch.Generator) -> torch.Tensor:
@@ -200,6 +216,17 @@ class RiffusionPipeline:
         from riffusion.vae_b200 import _Posterior
 
         return VAE_SCALE * _Posterior(mean, logvar).sample(generator=generator)
+
+    @staticmethod
+    def img2img_start(scheduler, num_inference_steps: int, strength: float) -> int:
+        """Index of the first timestep an img2img loop runs, `t_start`; noise is added at timesteps[t_start] and the loop
+        runs timesteps[t_start:].  The rule of `interpolate_img2img` (riffusion_pipeline.py:358-392):
+        init_timestep = min(int(steps * strength) + offset, steps), t_start = max(steps - init_timestep + offset, 0),
+        offset = the scheduler's `steps_offset` (1 for PNDM, 0 for DPM-Solver++).  For DPM-Solver++ this restates
+        diffusers' img2img pipeline from memory and is not pinned against diffusers (unpinned)."""
+        offset = scheduler.config.get("steps_offset", 0)
+        init_timestep = min(int(num_inference_steps * strength) + offset, num_inference_steps)
+        return max(num_inference_steps - init_timestep + offset, 0)
 
     # ------------------------------------------------------------------------------ denoising loop
     @torch.no_grad()
@@ -340,19 +367,8 @@ class RiffusionPipeline:
         sched = make_scheduler(scheduler)
         sched.set_timesteps(num_inference_steps)
         dev = self._device
-        do_cfg = guidance_scale > 1.0
-        text = self.embed_text(prompt) if text_embeddings is None else text_embeddings
-        text = text.to(device=dev, dtype=torch.float16)
-        text = text.expand(num_clips, -1, -1) if text.shape[0] == 1 else text
-        if text.shape[0] != num_clips:
-            raise ValueError(f"text_embeddings hold {text.shape[0]} rows for {num_clips} clips")
-        if do_cfg:
-            uncond = self.embed_text(negative_prompt or "") if uncond_embeddings is None else uncond_embeddings
-            uncond = uncond.to(device=dev, dtype=torch.float16)
-            uncond = uncond.expand(num_clips, -1, -1) if uncond.shape[0] == 1 else uncond
-            context = torch.cat([uncond, text]).contiguous()
-        else:
-            context = text.contiguous()
+        context = self._context(prompt, negative_prompt, num_clips, guidance_scale > 1.0, text_embeddings,
+                                uncond_embeddings)
         shape = (1, 4, height // 8, width // 8)
         if latents is None:
             latents = torch.cat([torch.randn(shape, generator=torch.Generator(device=self.device).manual_seed(seed + i),
@@ -362,11 +378,35 @@ class RiffusionPipeline:
             raise ValueError(f"latents must be {(num_clips,) + shape[1:]}, got {tuple(latents.shape)}")
         if sched.init_noise_sigma != 1.0:
             latents = (latents * sched.init_noise_sigma).contiguous()
+        latents, n_evals = self._denoise(sched, sched.timesteps, latents, context, guidance_scale)
+        return self._finish(latents, n_evals, output_type)
 
+    def _context(self, prompt: str, negative_prompt: T.Optional[str], n: int, do_cfg: bool,
+                 text_embeddings: T.Optional[torch.Tensor], uncond_embeddings: T.Optional[torch.Tensor]) -> torch.Tensor:
+        """[uncond | text] for n clips (text only without guidance): plain `embed_text` of the prompt and of the negative
+        prompt (default ""), or the injected embeddings (1 or n rows each)."""
+        dev = self._device
+        text = self.embed_text(prompt) if text_embeddings is None else text_embeddings
+        text = text.to(device=dev, dtype=torch.float16)
+        text = text.expand(n, -1, -1) if text.shape[0] == 1 else text
+        if text.shape[0] != n:
+            raise ValueError(f"text_embeddings hold {text.shape[0]} rows for {n} clips")
+        if not do_cfg:
+            return text.contiguous()
+        uncond = self.embed_text(negative_prompt or "") if uncond_embeddings is None else uncond_embeddings
+        uncond = uncond.to(device=dev, dtype=torch.float16)
+        uncond = uncond.expand(n, -1, -1) if uncond.shape[0] == 1 else uncond
+        return torch.cat([uncond, text]).contiguous()
+
+    def _denoise(self, sched, timesteps, latents: torch.Tensor, context: torch.Tensor,
+                 guidance_scale: float) -> T.Tuple[torch.Tensor, int]:
+        """The CFG loop of txt2img / img2img over `timesteps`: one UNet evaluation of [latents | latents] (a captured CUDA
+        graph when enabled) and one fused guidance + scheduler step each.  Returns (latents, evaluations)."""
+        do_cfg = guidance_scale > 1.0
         ctx_cache: T.Dict[str, T.Any] = {}
         graphed = self._graphed_unet(latents.shape, context) if do_cfg else None
         n_evals = 0
-        for t in sched.timesteps:
+        for t in timesteps:
             t_int = int(t)
             if graphed is not None:
                 eps_pair = graphed(latents, t_int)
@@ -377,7 +417,9 @@ class RiffusionPipeline:
             if not do_cfg:
                 eps_pair = torch.cat([eps_pair, eps_pair])
             latents = sched.step_cfg(eps_pair, guidance_scale if do_cfg else 0.0, t_int, latents)
+        return latents, n_evals
 
+    def _finish(self, latents: torch.Tensor, n_evals: int, output_type: T.Optional[str]) -> T.Dict[str, T.Any]:
         scaled = (1.0 / VAE_SCALE) * latents
         out: T.Dict[str, T.Any] = dict(latents=scaled, latents_unscaled=latents, n_unet_evals=n_evals)
         if output_type == "latent" or self.vae is None:
@@ -388,6 +430,60 @@ class RiffusionPipeline:
             out["images"] = [Image.fromarray(im) for im in ops.vae_image_to_u8(image).cpu().numpy()]
         else:
             out["images"] = (image / 2 + 0.5).clamp(0, 1).cpu().permute(0, 2, 3, 1).numpy()
+        return out
+
+    # ------------------------------------------------------------------------------ image -> image
+    @torch.no_grad()
+    def img2img(self, prompt: str, images: T.Union[torch.Tensor, T.Sequence[Image.Image]], *, strength: float = 0.55,
+                num_inference_steps: int = 25, guidance_scale: float = 7.0, negative_prompt: T.Optional[str] = None,
+                seed: int = 42, scheduler: str = "DPMSolverMultistepScheduler", output_type: T.Optional[str] = "pil",
+                text_embeddings: T.Optional[torch.Tensor] = None, uncond_embeddings: T.Optional[torch.Tensor] = None,
+                noise: T.Optional[torch.Tensor] = None,
+                moments: T.Optional[T.Tuple[torch.Tensor, torch.Tensor]] = None) -> T.Dict[str, T.Any]:
+        """Image to image: diffusers' StableDiffusionImg2ImgPipeline as the reference app calls it
+        (streamlit/util.py:354-396), for a batch of images in one CFG loop.
+
+        `images`: PIL images (preprocessed like `preprocess_image`) or a (B, 3, H, W) fp16 device tensor in [-1, 1]; H and
+        W must be multiples of 64.  Image i is denoised with its own generator seeded with `seed` (the app uses one seed
+        for every clip), which draws the VAE posterior noise (fp32) first and then the img2img noise (fp16).  The start
+        point follows `img2img_start` (unpinned for DPM-Solver++): noise is added at timesteps[t_start], then
+        timesteps[t_start:] are run.  `scheduler`: "DPMSolverMultistepScheduler" or "PNDMScheduler", a fresh instance per
+        call.  `text_embeddings` / `uncond_embeddings` / `noise` (B, 4, H/8, W/8) replace the text encoder and the
+        img2img noise draw; `moments` = (mean, logvar) replaces the VAE encoding of `images` (pass None for them).
+        Returns dict(images, latents (1/0.18215-scaled), latents_unscaled, n_unet_evals, t_start)."""
+        from riffusion.vae_b200 import _Posterior
+
+        sched = make_scheduler(scheduler)
+        sched.set_timesteps(num_inference_steps)
+        dev = self._device
+        if moments is None:
+            if not torch.is_tensor(images):
+                images = torch.cat([preprocess_image(im) for im in images])
+            images = images.to(device=dev, dtype=torch.float16)
+            if images.dim() != 4 or images.shape[1] != 3 or images.shape[2] % 64 or images.shape[3] % 64:
+                raise ValueError(f"images must be (B, 3, H, W) with H and W multiples of 64, got {tuple(images.shape)}")
+            moments = self.vae.encode_moments(images.contiguous())
+        mean, logvar = moments
+        n = mean.shape[0]
+        lats, draws = [], []
+        for i in range(n):
+            g = torch.Generator(device=self.device).manual_seed(seed)
+            lats.append(VAE_SCALE * _Posterior(mean[i:i + 1], logvar[i:i + 1]).sample(generator=g))
+            draws.append(torch.randn(lats[-1].shape, generator=g, device=self.device, dtype=torch.float16))
+        init_latents = torch.cat(lats).to(device=dev, dtype=torch.float16).contiguous()
+        noise = torch.cat(draws) if noise is None else noise.to(device=dev, dtype=torch.float16)
+        if noise.shape != init_latents.shape:
+            raise ValueError(f"noise must be {tuple(init_latents.shape)}, got {tuple(noise.shape)}")
+        do_cfg = guidance_scale > 1.0
+        context = self._context(prompt, negative_prompt, n, do_cfg, text_embeddings, uncond_embeddings)
+        t_start = self.img2img_start(sched, num_inference_steps, strength)
+        timesteps = sched.timesteps[t_start:]
+        latents = init_latents
+        if len(timesteps):
+            latents = sched.add_noise(init_latents, noise, int(timesteps[0]))
+        latents, n_evals = self._denoise(sched, timesteps, latents, context, guidance_scale)
+        out = self._finish(latents, n_evals, output_type)
+        out["t_start"] = t_start
         return out
 
     @torch.no_grad()
@@ -425,17 +521,122 @@ class RiffusionPipeline:
                           init_angles: T.Optional[torch.Tensor]) -> T.Tuple[torch.Tensor, torch.Tensor]:
         """VAE decode -> uint8 image (B, H, W, 3) -> mel amplitudes (B, channels, H, W) -> waveform (B, channels, L),
         without leaving the device."""
-        from riffusion import _native
-
         image = self.vae.decode(scaled_latents).sample
         u8 = ops.vae_image_to_u8(image)
+        return u8, self._u8_to_waveform(u8, converter, stereo, init_angles)
+
+    @staticmethod
+    def _u8_to_waveform(u8: torch.Tensor, converter, stereo: bool, init_angles: T.Optional[torch.Tensor]) -> torch.Tensor:
+        """uint8 images (B, H, W, 3) -> mel amplitudes (B, channels, H, W) -> waveform (B, channels, L)."""
+        from riffusion import _native
+
         B, H, W, _ = u8.shape
         mel = torch.empty((B, 2 if stereo else 1, H, W), dtype=torch.float32, device=u8.device)
         p = converter.p
         for i in range(B):
             _native.call("rf_image_to_mel", u8.device, u8[i].data_ptr(), H, W, int(stereo), float(p.power_for_image),
                          30e6, mel[i].data_ptr())
-        return u8, converter.waveform_from_mel_amplitudes(mel, init_angles)
+        return converter.waveform_from_mel_amplitudes(mel, init_angles)
+
+    # ------------------------------------------------------------------------------ audio -> audio
+    @torch.no_grad()
+    def audio_to_audio(self, track, prompt: str, *, params=None, start_time_s: float = 0.0, duration_s: float = 20.0,
+                       clip_duration_s: float = 5.0, overlap_duration_s: float = 0.2,
+                       negative_prompt: T.Optional[str] = None, seed: int = 42, denoising: float = 0.55,
+                       num_inference_steps: int = 25, guidance_scale: float = 7.0,
+                       scheduler: str = "DPMSolverMultistepScheduler", prompt_b: T.Optional[str] = None,
+                       seed_b: T.Optional[int] = None, denoising_b: T.Optional[float] = None, max_batch: int = 32,
+                       init_angles: T.Optional[torch.Tensor] = None, apply_filters: bool = True,
+                       text_embeddings: T.Optional[torch.Tensor] = None,
+                       uncond_embeddings: T.Optional[torch.Tensor] = None, converter=None) -> T.Dict[str, T.Any]:
+        """Riff a whole track: the reference app's Audio to Audio task (streamlit/tasks/audio_to_audio.py:86-330).
+
+        The track (an AudioSegment at params.sample_rate) is cut into overlapping clips (`audio_to_audio.clip_start_times`,
+        `slice_audio_into_clips`).  On the device, per batch of at most `max_batch` clips: waveform -> mel -> uint8 image
+        (per-clip max, `spectrogram_image_from_audio`), bicubic resize to a 32-pixel stride -> VAE encode -> img2img ->
+        VAE decode -> uint8 -> bicubic resize back -> mel -> waveform.  On the host: peak-normalised int16,
+        `apply_filters` and `stitch_segments` with an `overlap_duration_s` crossfade.
+
+        `params` defaults to mono 0-10 kHz.  Without `prompt_b` every clip runs `img2img` (prompt, negative prompt,
+        `denoising` as strength, `seed` for every clip, `scheduler`).  With `prompt_b` it is the interpolation mode: clip i
+        of n is `riffuse_batch` of InferenceInput(alpha = linspace(0, 1, n)[i], start = (prompt, seed, denoising),
+        end = (prompt_b, seed_b, denoising_b)) - PNDM, weighted prompts, no negative prompt.  `init_angles` (clips,
+        channels, n_fft/2 + 1, frames) fixes Griffin-Lim's initial phases; `text_embeddings` / `uncond_embeddings`
+        replace the text encoder of the img2img mode.
+
+        Returns dict(segment (the stitched AudioSegment), source_images and images ((clips, H, W, 3) uint8 device tensors
+        before and after denoising), denoised_images (the decoded images at the 32-stride size), clip_start_times (s), waveform ((clips, channels, L) fp32, before normalisation),
+        n_unet_evals (per batch))."""
+        from riffusion import audio_to_audio as a2a
+        from riffusion.datatypes import PromptInput
+        from riffusion.spectrogram_converter import SpectrogramConverter
+        from riffusion.spectrogram_image_converter import _conform_channels
+        from riffusion.spectrogram_params import SpectrogramParams
+        from riffusion.util import audio_util, image_util
+
+        if params is None:
+            params = SpectrogramParams(min_frequency=0, max_frequency=10000, stereo=False)
+        if max_batch < 1:
+            raise ValueError("max_batch must be at least 1")
+        if track.frame_rate != params.sample_rate:
+            track = track.set_frame_rate(params.sample_rate)        # the app resamples (audio_to_audio.py:89-91)
+        starts = a2a.clip_start_times(track.duration_seconds, start_time_s, duration_s, clip_duration_s,
+                                      overlap_duration_s)
+        if len(starts) == 0:
+            raise ValueError(f"no {clip_duration_s} s clip fits in {track.duration_seconds:.2f} s of audio from "
+                             f"{start_time_s} s (duration {duration_s} s): the track is shorter than one clip")
+        frames = a2a.clip_frames(clip_duration_s, params.sample_rate, params.hop_length)
+        width, height = a2a.stride_32_size(frames, params.num_frequencies)
+        a2a.check_denoising_size(width, height, clip_duration_s)
+        if converter is None:
+            converter = SpectrogramConverter(params, device=self.device)
+        if converter.p != params:
+            raise ValueError("converter was built for other SpectrogramParams")
+
+        clips = [_conform_channels(c, params.stereo) for c in a2a.slice_audio_into_clips(track, starts, clip_duration_s)]
+        waves = np.stack([np.array([c.get_array_of_samples() for c in clip.split_to_mono()]) for clip in clips])
+        waves = torch.from_numpy(waves.astype(np.float32)).to(self._device)           # (clips, channels, samples)
+        n = waves.shape[0]
+        if prompt_b is not None:
+            alphas = np.linspace(0, 1, n)
+            a = PromptInput(prompt=prompt, seed=seed, denoising=denoising, guidance=guidance_scale)
+            b = PromptInput(prompt=prompt_b, seed=seed if seed_b is None else seed_b,
+                            denoising=denoising if denoising_b is None else denoising_b, guidance=guidance_scale)
+            requests = [InferenceInput(start=a, end=b, alpha=float(al), num_inference_steps=num_inference_steps)
+                        for al in alphas]
+        sources, denoised, riffed, out_waves, n_evals = [], [], [], [], []
+        for lo in range(0, n, max_batch):
+            hi = min(n, lo + max_batch)
+            mel = converter.mel_amplitudes_from_waveform(waves[lo:hi])                 # (b, channels, H, frames)
+            src = torch.stack([image_util.image_from_spectrogram_device(m, power=params.power_for_image)[0] for m in mel])
+            Hs, Ws = src.shape[1], src.shape[2]
+            _, vae_in = ops.resize_bicubic_u8(src, width, height, want_f16=True)
+            moments = self.vae.encode_moments(vae_in)
+            if prompt_b is None:
+                out = self.img2img(prompt, None, strength=denoising, num_inference_steps=num_inference_steps,
+                                   guidance_scale=guidance_scale, negative_prompt=negative_prompt, seed=seed,
+                                   scheduler=scheduler, output_type="latent", text_embeddings=text_embeddings,
+                                   uncond_embeddings=uncond_embeddings, moments=moments)
+                latents = out["latents"]
+                n_evals.append(out["n_unet_evals"])
+            else:
+                latents = torch.cat(self.riffuse_batch(requests[lo:hi], None, moments=moments, output_type="latent"))
+            u8 = ops.vae_image_to_u8(self.vae.decode(latents).sample)
+            back, _ = ops.resize_bicubic_u8(u8, Ws, Hs)
+            angles = None if init_angles is None else init_angles[lo:hi]
+            out_waves.append(self._u8_to_waveform(back, converter, params.stereo, angles))
+            sources.append(src)
+            denoised.append(u8)
+            riffed.append(back)
+        waveform = torch.cat(out_waves)
+        segments = []
+        for w in waveform.cpu().numpy():
+            seg = audio_util.audio_from_waveform(samples=w, sample_rate=params.sample_rate, normalize=True)
+            segments.append(audio_util.apply_filters(seg, compression=False) if apply_filters else seg)
+        return dict(segment=audio_util.stitch_segments(segments, crossfade_s=overlap_duration_s),
+                    source_images=torch.cat(sources), denoised_images=torch.cat(denoised), images=torch.cat(riffed),
+                    clip_start_times=starts,
+                    waveform=waveform, n_unet_evals=n_evals)
 
     # ------------------------------------------------------------------------------ batched request -> audio
     @torch.no_grad()

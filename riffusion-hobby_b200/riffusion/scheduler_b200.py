@@ -146,8 +146,15 @@ class DPMSolverMultistepSchedulerB200:
     def scale_model_input(self, sample: torch.Tensor, timestep=None) -> torch.Tensor:
         return sample
 
+    def add_noise(self, original: torch.Tensor, noise: torch.Tensor, timestep) -> torch.Tensor:
+        """img2img start point sqrt(ab_t) x + sqrt(1 - ab_t) noise, with the coefficients PNDM's add_noise uses."""
+        a = float(self.alphas_cumprod[int(timestep)])
+        return ops.axpby(original.contiguous(), noise.contiguous(), a ** 0.5, (1.0 - a) ** 0.5)
+
     def plan(self, timestep: int):
-        """Host bookkeeping of one step: (order, (alpha_s0, sigma_s0, c_x, c_0, c_1)) in fp64."""
+        """Host bookkeeping of one step: (order, (alpha_s0, sigma_s0, c_x, c_0, c_1)) in fp64.  A loop that starts
+        mid-schedule (img2img) is first order on its first step (no history yet); the `lower_order_final` rule for the
+        last step looks at the whole schedule's length."""
         ts = self.timesteps.tolist()
         timestep = int(timestep)
         i = ts.index(timestep) if timestep in ts else len(ts) - 1

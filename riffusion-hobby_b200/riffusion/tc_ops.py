@@ -339,6 +339,39 @@ def vae_image_to_u8(x_nchw: torch.Tensor) -> torch.Tensor:
     return y
 
 
+def resize_bicubic_u8(x_nhwc: torch.Tensor, width: int, height: int,
+                      want_f16: bool = False) -> T.Tuple[torch.Tensor, T.Optional[torch.Tensor]]:
+    """PIL `Image.resize((width, height), Image.BICUBIC)` of every image of a (B, H, W, C) uint8 batch, bit-exact.
+    Returns the (B, height, width, C) uint8 batch and, with `want_f16`, the same pixels as the VAE input
+    (B, C, height, width) fp16 = 2 * (u8 / 255) - 1 (`preprocess_image`'s arithmetic)."""
+    if not x_nhwc.is_cuda or x_nhwc.dtype != torch.uint8 or x_nhwc.dim() != 4:
+        raise _native.NativeError(f"x must be a (B, H, W, C) CUDA uint8 tensor (got {x_nhwc.dtype} {tuple(x_nhwc.shape)} "
+                                  f"on {x_nhwc.device})")
+    x = x_nhwc.contiguous()
+    B, H, W, Cc = x.shape
+    y = torch.empty((B, height, width, Cc), dtype=torch.uint8, device=x.device)
+    f16 = torch.empty((B, Cc, height, width), dtype=torch.float16, device=x.device) if want_f16 else None
+    nbytes = _native.lib().rf_resize_bicubic_workspace_bytes(B, H, W, Cc, height, width)
+    ws = torch.empty(max(int(nbytes), 1), dtype=torch.uint8, device=x.device)
+    _native.call("rf_resize_bicubic_u8", x.device, x.data_ptr(), B, H, W, Cc, height, width, y.data_ptr(),
+                 _native.ptr(f16), ws.data_ptr(), int(nbytes))
+    return y, f16
+
+
+def resize_bicubic_table(in_size: int, out_size: int):
+    """The host tap table of an in_size -> out_size bicubic resize, as the device passes read it: (first, count, taps)
+    with first / count (out_size,) int32 and taps (out_size, n_taps) int32 with 22 fractional bits."""
+    import numpy as np
+
+    lib = _native.lib()
+    taps = lib.rf_resize_bicubic_taps(in_size, out_size)
+    if taps <= 0:
+        _native.check(1)
+    tab = np.empty((out_size, 2 + taps), dtype=np.int32)
+    _native.check(lib.rf_resize_bicubic_table(in_size, out_size, tab.ctypes.data, tab.nbytes))
+    return tab[:, 0].copy(), tab[:, 1].copy(), tab[:, 2:].copy()
+
+
 def slerp(alphas, v0: torch.Tensor, v1: torch.Tensor, dot_threshold: float = 0.9995) -> torch.Tensor:
     """Per-sample spherical interpolation on the device.  v0, v1: (B, ...) fp16; alphas: float or sequence of B floats."""
     _f16(v0, "v0"), _f16(v1, "v1")
