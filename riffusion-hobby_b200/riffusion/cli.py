@@ -53,6 +53,20 @@ def _store_image(picture: Image.Image, path, fmt: str) -> None:
     picture.save(path, exif=picture.getexif(), format=fmt)
 
 
+def _store_spectrogram(pixels: np.ndarray, params: SpectrogramParams, path, fmt: str = "PNG") -> None:
+    """Save a (H, W, 3) uint8 spectrogram image with `params` in its EXIF block."""
+    picture = Image.fromarray(pixels)
+    picture.getexif().update(params.to_exif().items())
+    _store_image(picture, path, fmt)
+
+
+def _app_params(use_20k: bool) -> SpectrogramParams:
+    """The app's "Use 20kHz" switch: stereo 10 Hz - 20 kHz, else mono 0 - 10 kHz."""
+    if use_20k:
+        return SpectrogramParams(min_frequency=10, max_frequency=20000, stereo=True)
+    return SpectrogramParams(min_frequency=0, max_frequency=10000, stereo=False)
+
+
 def _files_in(folder: str, pattern: str = "*", limit: int = -1) -> T.List[Path]:
     found = sorted(p for p in Path(folder).glob(pattern) if p.is_file())
     return found[:limit] if limit > 0 else found
@@ -192,10 +206,7 @@ def text_to_audio(*, prompt: str, audio: str, image: str = "", negative_prompt: 
     from riffusion.riffusion_pipeline import RiffusionPipeline
     from riffusion.util import audio_util
 
-    if use_20k:         # the app's "Use 20kHz" switch
-        params = SpectrogramParams(min_frequency=10, max_frequency=20000, stereo=True)
-    else:
-        params = SpectrogramParams(min_frequency=0, max_frequency=10000, stereo=False)
+    params = _app_params(use_20k)
     pipe = RiffusionPipeline.load_checkpoint(checkpoint=checkpoint, device=device)
     out = pipe.text_to_audio(prompt, params=params, negative_prompt=negative_prompt or None, seed=seed,
                              num_clips=num_clips, num_inference_steps=num_inference_steps, guidance_scale=guidance,
@@ -214,10 +225,8 @@ def text_to_audio(*, prompt: str, audio: str, image: str = "", negative_prompt: 
         segment.export(str(wav_path), format=wav_path.suffix[1:])
         print(f"Wrote {wav_path} ({segment.duration_seconds:.2f} seconds)")
         if image:
-            picture = Image.fromarray(images[i])
-            picture.getexif().update(params.to_exif().items())
             img_path = target(image, i)
-            _store_image(picture, img_path, _PIL_FORMAT.get(img_path.suffix[1:].lower(), "PNG"))
+            _store_spectrogram(images[i], params, img_path, _PIL_FORMAT.get(img_path.suffix[1:].lower(), "PNG"))
             print(f"Wrote {img_path}")
 
 
@@ -231,10 +240,7 @@ def audio_to_audio(*, audio: str, output: str, prompt: str, image_dir: str = "",
     interpolate from --prompt to --prompt-b along the track (--seed-b / --denoising-b: -1 = same as the first end)."""
     from riffusion.riffusion_pipeline import RiffusionPipeline
 
-    if use_20k:         # the app's "Use 20kHz" switch
-        params = SpectrogramParams(min_frequency=10, max_frequency=20000, stereo=True)
-    else:
-        params = SpectrogramParams(min_frequency=0, max_frequency=10000, stereo=False)
+    params = _app_params(use_20k)
     track = AudioSegment.from_file(audio)
     pipe = RiffusionPipeline.load_checkpoint(checkpoint=checkpoint, device=device)
     out = pipe.audio_to_audio(
@@ -252,9 +258,7 @@ def audio_to_audio(*, audio: str, output: str, prompt: str, image_dir: str = "",
         for kind in ("source", "riffed"):
             images = out["source_images" if kind == "source" else "images"].cpu().numpy()
             for i, im in enumerate(images):
-                picture = Image.fromarray(im)
-                picture.getexif().update(params.to_exif().items())
-                _store_image(picture, target / f"clip_{i}_{kind}.png", "PNG")
+                _store_spectrogram(im, params, target / f"clip_{i}_{kind}.png")
         print(f"Wrote {2 * len(images)} images to {image_dir}")
 
 

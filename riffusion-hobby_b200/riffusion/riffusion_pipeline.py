@@ -15,7 +15,6 @@ encoder is supplied, otherwise callers pass text embeddings directly.
 from __future__ import annotations
 
 import functools
-import inspect
 import typing as T
 from pathlib import Path
 
@@ -26,11 +25,14 @@ from PIL import Image
 from riffusion import tc_ops as ops
 from riffusion.datatypes import InferenceInput
 from riffusion.scheduler_b200 import PNDMSchedulerB200, make_scheduler
+from riffusion.spectrogram_params import SpectrogramParams
 from riffusion.unet_b200 import UNetB200
 from riffusion.util import torch_util
-from riffusion.vae_b200 import VaeB200
+from riffusion.vae_b200 import VaeB200, _Posterior
 
 VAE_SCALE = 0.18215
+# the spectrogram parameters of text_to_audio / audio_to_audio when none are given: the app's mono 0-10 kHz
+DEFAULT_PARAMS = SpectrogramParams(min_frequency=0, max_frequency=10000, stereo=False)
 
 
 class RiffusionPipeline:
@@ -159,7 +161,6 @@ class RiffusionPipeline:
             assert len(images) == len(inputs)
         else:
             assert init_images is None and moments[0].shape[0] == len(inputs)
-        from riffusion.vae_b200 import _Posterior
         embed = self.embed_text_weighted if use_reweighting else self.embed_text
         groups: T.Dict[T.Tuple, T.List[int]] = {}
         for i, inp in enumerate(inputs):
@@ -184,8 +185,7 @@ class RiffusionPipeline:
                 if moments is None:
                     lats.append(self.encode_image(images[i], g_post))
                 else:
-                    post = _Posterior(moments[0][i:i + 1], moments[1][i:i + 1])
-                    lats.append(VAE_SCALE * post.sample(generator=g_post))
+                    lats.append(_sample_latents(moments[0][i:i + 1], moments[1][i:i + 1], g_post))
                 ga = torch.Generator(device=self.device).manual_seed(inp.start.seed)
                 gb = torch.Generator(device=self.device).manual_seed(inp.end.seed)
                 shape = lats[-1].shape
@@ -213,20 +213,24 @@ class RiffusionPipeline:
             img = preprocess_image(init_image).to(device=self.device, dtype=torch.float16)
             self._moment_cache[key] = self.vae.encode_moments(img)
         mean, logvar = self._moment_cache[key]
-        from riffusion.vae_b200 import _Posterior
-
-        return VAE_SCALE * _Posterior(mean, logvar).sample(generator=generator)
+        return _sample_latents(mean, logvar, generator)
 
     @staticmethod
     def img2img_start(scheduler, num_inference_steps: int, strength: float) -> int:
-        """Index of the first timestep an img2img loop runs, `t_start`; noise is added at timesteps[t_start] and the loop
-        runs timesteps[t_start:].  The rule of `interpolate_img2img` (riffusion_pipeline.py:358-392):
+        """Index of the first timestep an img2img loop runs, `t_start`; `img2img` adds noise at timesteps[t_start] and
+        runs timesteps[t_start:].  The rule of `interpolate_img2img`, see `_img2img_steps`.  For DPM-Solver++ this
+        restates diffusers' img2img pipeline from memory and is not pinned against diffusers (unpinned)."""
+        return RiffusionPipeline._img2img_steps(scheduler, num_inference_steps, strength)[1]
+
+    @staticmethod
+    def _img2img_steps(scheduler, num_inference_steps: int, strength: float) -> T.Tuple[int, int]:
+        """(init_timestep, t_start) of `interpolate_img2img` (riffusion_pipeline.py:358-392):
         init_timestep = min(int(steps * strength) + offset, steps), t_start = max(steps - init_timestep + offset, 0),
-        offset = the scheduler's `steps_offset` (1 for PNDM, 0 for DPM-Solver++).  For DPM-Solver++ this restates
-        diffusers' img2img pipeline from memory and is not pinned against diffusers (unpinned)."""
+        offset = the scheduler's step offset (1 for PNDM, 0 for DPM-Solver++).  `interpolate_img2img` adds noise at
+        timesteps[-init_timestep], which is timesteps[t_start] whenever the loop runs at least one step."""
         offset = scheduler.config.get("steps_offset", 0)
         init_timestep = min(int(num_inference_steps * strength) + offset, num_inference_steps)
-        return max(num_inference_steps - init_timestep + offset, 0)
+        return init_timestep, max(num_inference_steps - init_timestep + offset, 0)
 
     # ------------------------------------------------------------------------------ denoising loop
     @torch.no_grad()
@@ -243,7 +247,8 @@ class RiffusionPipeline:
         let callers inject what the reference computes internally (CLIP("") and the generator draws) — used by
         the parity tests and by runs without a text encoder."""
         batch_size = text_embeddings.shape[0]
-        self.scheduler.set_timesteps(num_inference_steps)
+        sched = self.scheduler
+        sched.set_timesteps(num_inference_steps)
         dev = self._device
         text_embeddings = text_embeddings.to(device=dev, dtype=torch.float16)
         bs_embed, seq_len, _ = text_embeddings.shape
@@ -265,17 +270,16 @@ class RiffusionPipeline:
                 ids = self.tokenizer(uncond_tokens, padding="max_length", max_length=self.tokenizer.model_max_length,
                                      truncation=True, return_tensors="pt").input_ids
                 uncond_embeddings = self.text_encoder(ids.to(self.device))[0]
-            uncond_embeddings = uncond_embeddings.to(device=dev, dtype=torch.float16)
-            uncond_embeddings = uncond_embeddings.repeat_interleave(batch_size * num_images_per_prompt // uncond_embeddings.shape[0], dim=0)
-            context = torch.cat([uncond_embeddings, text_embeddings]).contiguous()              # :354
-        else:
-            context = text_embeddings.contiguous()
+            if num_images_per_prompt > 1 and uncond_embeddings.shape[0] == batch_size:
+                # one row per prompt, repeated like the text rows above (:347-350)
+                uncond_embeddings = uncond_embeddings.repeat_interleave(num_images_per_prompt, dim=0)
+        context = self._context(None, None, batch_size * num_images_per_prompt, do_cfg, text_embeddings,
+                                uncond_embeddings)                                                 # :354
 
         latents_dtype = torch.float16
         strength = (1 - interpolate_alpha) * strength_a + interpolate_alpha * strength_b          # :358
-        offset = self.scheduler.config.get("steps_offset", 0)
-        init_timestep = min(int(num_inference_steps * strength) + offset, num_inference_steps)    # :361-363
-        t_noise = int(self.scheduler.timesteps[-init_timestep])                                   # :365
+        init_timestep, t_start = self._img2img_steps(sched, num_inference_steps, strength)        # :361-363, :392
+        t_noise = int(sched.timesteps[-init_timestep])                                            # :365
         init_latents = init_latents.to(device=dev, dtype=latents_dtype).contiguous()
         if noise is None:
             if noise_a is None:
@@ -287,46 +291,12 @@ class RiffusionPipeline:
             else:                      # the reference's host-numpy slerp in fp16 (bit-compatible)
                 noise = torch_util.slerp(interpolate_alpha, noise_a.to(dev, latents_dtype), noise_b.to(dev, latents_dtype))
         noise = noise.to(dev, latents_dtype).contiguous()
-        init_latents_orig = init_latents
-        latents = self.scheduler.add_noise(init_latents, noise, t_noise)                           # :379
-
-        accepts_eta = "eta" in set(inspect.signature(self.scheduler.step).parameters.keys())       # PNDM ignores eta
-        del accepts_eta
-        t_start = max(num_inference_steps - init_timestep + offset, 0)                             # :392
-        timesteps = self.scheduler.timesteps[t_start:]
-        ctx_cache: T.Dict[str, T.Any] = {}
-        graphed = self._graphed_unet(latents.shape, context) if do_cfg else None
-        n_evals = 0
-        for t in timesteps:                                                                        # :398
-            t_int = int(t)
-            if graphed is not None:
-                eps_pair = graphed(latents, t_int)
-            else:
-                model_in = torch.cat([latents] * 2) if do_cfg else latents                         # :400-403
-                eps_pair = self.unet(model_in, t_int, encoder_hidden_states=context, ctx_cache=ctx_cache).sample
-            n_evals += 1
-            if not do_cfg:
-                eps_pair = torch.cat([eps_pair, eps_pair])
-            latents = self.scheduler.step_cfg(eps_pair, guidance_scale if do_cfg else 0.0, t_int, latents)   # :411-418
-            if mask is not None:                                                                   # :420-425
-                m = mask.to(device=dev, dtype=latents_dtype).expand_as(latents).contiguous()
-                latents = self.scheduler.add_noise(init_latents_orig, noise, t_int, mask=m, blend_with=latents)
-
-        # :427 — the reference rescales in fp16 (`1.0 / 0.18215 * latents`) and returns THAT tensor under "latents"; the
-        # un-scaled loop state and the evaluation count are extra keys of this implementation
-        scaled = (1.0 / VAE_SCALE) * latents
-        out: T.Dict[str, T.Any] = dict(latents=scaled, nsfw_content_detected=False, latents_unscaled=latents,
-                                       n_unet_evals=n_evals)
-        if output_type == "latent" or self.vae is None:
-            out["images"] = None
-            return out
-        image = self.vae.decode(scaled).sample                                                       # :428
-        if output_type == "pil":
-            # :430-434 `(image / 2 + 0.5).clamp(0, 1)` -> numpy_to_pil, in the fp16 arithmetic of the reference's CUDA path
-            u8 = ops.vae_image_to_u8(image).cpu().numpy()
-            out["images"] = [Image.fromarray(im) for im in u8]
-        else:
-            out["images"] = (image / 2 + 0.5).clamp(0, 1).cpu().permute(0, 2, 3, 1).numpy()         # float16 array, like the reference
+        latents = sched.add_noise(init_latents, noise, t_noise)                                    # :379
+        latents, n_evals = self._denoise(sched, sched.timesteps[t_start:], latents, context, guidance_scale,
+                                         mask=mask, init=init_latents, noise=noise)                # :398-425
+        # :427-436 — "latents" is the 1/0.18215-scaled tensor, as the reference returns it
+        out = self._finish(latents, n_evals, output_type)
+        out["nsfw_content_detected"] = False
         return out
 
     def _graphed_unet(self, latent_shape, context: torch.Tensor):
@@ -386,25 +356,32 @@ class RiffusionPipeline:
         """[uncond | text] for n clips (text only without guidance): plain `embed_text` of the prompt and of the negative
         prompt (default ""), or the injected embeddings (1 or n rows each)."""
         dev = self._device
-        text = self.embed_text(prompt) if text_embeddings is None else text_embeddings
-        text = text.to(device=dev, dtype=torch.float16)
-        text = text.expand(n, -1, -1) if text.shape[0] == 1 else text
-        if text.shape[0] != n:
-            raise ValueError(f"text_embeddings hold {text.shape[0]} rows for {n} clips")
+
+        def rows(emb: torch.Tensor, name: str) -> torch.Tensor:
+            emb = emb.to(device=dev, dtype=torch.float16)
+            emb = emb.expand(n, -1, -1) if emb.shape[0] == 1 else emb
+            if emb.shape[0] != n:
+                raise ValueError(f"{name} hold {emb.shape[0]} rows for {n} clips")
+            return emb
+
+        text = rows(self.embed_text(prompt) if text_embeddings is None else text_embeddings, "text_embeddings")
         if not do_cfg:
             return text.contiguous()
         uncond = self.embed_text(negative_prompt or "") if uncond_embeddings is None else uncond_embeddings
-        uncond = uncond.to(device=dev, dtype=torch.float16)
-        uncond = uncond.expand(n, -1, -1) if uncond.shape[0] == 1 else uncond
-        return torch.cat([uncond, text]).contiguous()
+        return torch.cat([rows(uncond, "uncond_embeddings"), text]).contiguous()
 
-    def _denoise(self, sched, timesteps, latents: torch.Tensor, context: torch.Tensor,
-                 guidance_scale: float) -> T.Tuple[torch.Tensor, int]:
-        """The CFG loop of txt2img / img2img over `timesteps`: one UNet evaluation of [latents | latents] (a captured CUDA
-        graph when enabled) and one fused guidance + scheduler step each.  Returns (latents, evaluations)."""
+    def _denoise(self, sched, timesteps, latents: torch.Tensor, context: torch.Tensor, guidance_scale: float,
+                 mask: T.Optional[torch.Tensor] = None, init: T.Optional[torch.Tensor] = None,
+                 noise: T.Optional[torch.Tensor] = None) -> T.Tuple[torch.Tensor, int]:
+        """The CFG loop over `timesteps`: one UNet evaluation of [latents | latents] (a captured CUDA graph when enabled)
+        and one fused guidance + scheduler step each.  With a `mask`, every step is followed by the inpainting blend of
+        interpolate_img2img (:420-425): `init` noised with `noise` at that step's timestep where the mask is 1, the
+        stepped latents where it is 0.  Returns (latents, evaluations)."""
         do_cfg = guidance_scale > 1.0
         ctx_cache: T.Dict[str, T.Any] = {}
         graphed = self._graphed_unet(latents.shape, context) if do_cfg else None
+        if mask is not None:
+            mask = mask.to(device=latents.device, dtype=latents.dtype).expand_as(latents).contiguous()
         n_evals = 0
         for t in timesteps:
             t_int = int(t)
@@ -417,20 +394,28 @@ class RiffusionPipeline:
             if not do_cfg:
                 eps_pair = torch.cat([eps_pair, eps_pair])
             latents = sched.step_cfg(eps_pair, guidance_scale if do_cfg else 0.0, t_int, latents)
+            if mask is not None:
+                latents = sched.add_noise(init, noise, t_int, mask=mask, blend_with=latents)
         return latents, n_evals
 
     def _finish(self, latents: torch.Tensor, n_evals: int, output_type: T.Optional[str]) -> T.Dict[str, T.Any]:
+        """dict(latents (1/0.18215-scaled), latents_unscaled, n_unet_evals, images): PIL images, a float16 (B, H, W, 3)
+        array in [0, 1] for any other output_type, or None for "latent" and without a VAE."""
         scaled = (1.0 / VAE_SCALE) * latents
         out: T.Dict[str, T.Any] = dict(latents=scaled, latents_unscaled=latents, n_unet_evals=n_evals)
         if output_type == "latent" or self.vae is None:
             out["images"] = None
-            return out
-        image = self.vae.decode(scaled).sample
-        if output_type == "pil":
-            out["images"] = [Image.fromarray(im) for im in ops.vae_image_to_u8(image).cpu().numpy()]
+        elif output_type == "pil":
+            out["images"] = [Image.fromarray(im) for im in self._decode_u8(scaled).cpu().numpy()]
         else:
+            image = self.vae.decode(scaled).sample
             out["images"] = (image / 2 + 0.5).clamp(0, 1).cpu().permute(0, 2, 3, 1).numpy()
         return out
+
+    def _decode_u8(self, scaled_latents: torch.Tensor) -> torch.Tensor:
+        """VAE decode -> (B, H, W, 3) uint8 images: `(image / 2 + 0.5).clamp(0, 1)` -> numpy_to_pil (:430-434) in the fp16
+        arithmetic of the reference's CUDA path, on the device."""
+        return ops.vae_image_to_u8(self.vae.decode(scaled_latents).sample)
 
     # ------------------------------------------------------------------------------ image -> image
     @torch.no_grad()
@@ -451,8 +436,6 @@ class RiffusionPipeline:
         call.  `text_embeddings` / `uncond_embeddings` / `noise` (B, 4, H/8, W/8) replace the text encoder and the
         img2img noise draw; `moments` = (mean, logvar) replaces the VAE encoding of `images` (pass None for them).
         Returns dict(images, latents (1/0.18215-scaled), latents_unscaled, n_unet_evals, t_start)."""
-        from riffusion.vae_b200 import _Posterior
-
         sched = make_scheduler(scheduler)
         sched.set_timesteps(num_inference_steps)
         dev = self._device
@@ -465,17 +448,16 @@ class RiffusionPipeline:
             moments = self.vae.encode_moments(images.contiguous())
         mean, logvar = moments
         n = mean.shape[0]
+        context = self._context(prompt, negative_prompt, n, guidance_scale > 1.0, text_embeddings, uncond_embeddings)
         lats, draws = [], []
         for i in range(n):
             g = torch.Generator(device=self.device).manual_seed(seed)
-            lats.append(VAE_SCALE * _Posterior(mean[i:i + 1], logvar[i:i + 1]).sample(generator=g))
+            lats.append(_sample_latents(mean[i:i + 1], logvar[i:i + 1], g))
             draws.append(torch.randn(lats[-1].shape, generator=g, device=self.device, dtype=torch.float16))
         init_latents = torch.cat(lats).to(device=dev, dtype=torch.float16).contiguous()
         noise = torch.cat(draws) if noise is None else noise.to(device=dev, dtype=torch.float16)
         if noise.shape != init_latents.shape:
             raise ValueError(f"noise must be {tuple(init_latents.shape)}, got {tuple(noise.shape)}")
-        do_cfg = guidance_scale > 1.0
-        context = self._context(prompt, negative_prompt, n, do_cfg, text_embeddings, uncond_embeddings)
         t_start = self.img2img_start(sched, num_inference_steps, strength)
         timesteps = sched.timesteps[t_start:]
         latents = init_latents
@@ -498,32 +480,29 @@ class RiffusionPipeline:
         -> inverse mel + Griffin-Lim.  `params` defaults to mono 0-10 kHz.  Returns device tensors: images (B, H, W, 3)
         uint8, waveform (B, channels, hop * (W - 1)) fp32 before peak normalisation, latents, latents_unscaled,
         n_unet_evals."""
-        from riffusion.spectrogram_converter import SpectrogramConverter
-        from riffusion.spectrogram_params import SpectrogramParams
-
-        if params is None:
-            params = SpectrogramParams(min_frequency=0, max_frequency=10000, stereo=False)
+        params = DEFAULT_PARAMS if params is None else params
         if height is not None and height != params.num_frequencies:
             raise ValueError(f"height {height} differs from params.num_frequencies {params.num_frequencies}")
-        if converter is None:
-            converter = SpectrogramConverter(params, device=self.device)
-        if converter.p != params:
-            raise ValueError("converter was built for other SpectrogramParams")
+        converter = self._converter(params, converter)
         out = self.txt2img(prompt, negative_prompt=negative_prompt, seed=seed, num_clips=num_clips,
                            num_inference_steps=num_inference_steps, guidance_scale=guidance_scale, width=width,
                            height=params.num_frequencies, scheduler=scheduler, output_type="latent",
                            text_embeddings=text_embeddings, uncond_embeddings=uncond_embeddings, latents=latents)
-        u8, wave = self._latents_to_audio(out["latents"], converter, params.stereo, init_angles)
+        u8 = self._decode_u8(out["latents"])
+        wave = self._u8_to_waveform(u8, converter, params.stereo, init_angles)
         return dict(images=u8, waveform=wave, latents=out["latents"], latents_unscaled=out["latents_unscaled"],
                     n_unet_evals=out["n_unet_evals"])
 
-    def _latents_to_audio(self, scaled_latents: torch.Tensor, converter, stereo: bool,
-                          init_angles: T.Optional[torch.Tensor]) -> T.Tuple[torch.Tensor, torch.Tensor]:
-        """VAE decode -> uint8 image (B, H, W, 3) -> mel amplitudes (B, channels, H, W) -> waveform (B, channels, L),
-        without leaving the device."""
-        image = self.vae.decode(scaled_latents).sample
-        u8 = ops.vae_image_to_u8(image)
-        return u8, self._u8_to_waveform(u8, converter, stereo, init_angles)
+    def _converter(self, params, converter):
+        """`converter`, which must have been built for `params`, or a new SpectrogramConverter for them on this
+        pipeline's device."""
+        from riffusion.spectrogram_converter import SpectrogramConverter
+
+        if converter is None:
+            converter = SpectrogramConverter(params, device=self.device)
+        if converter.p != params:
+            raise ValueError("converter was built for other SpectrogramParams")
+        return converter
 
     @staticmethod
     def _u8_to_waveform(u8: torch.Tensor, converter, stereo: bool, init_angles: T.Optional[torch.Tensor]) -> torch.Tensor:
@@ -569,13 +548,10 @@ class RiffusionPipeline:
         n_unet_evals (per batch))."""
         from riffusion import audio_to_audio as a2a
         from riffusion.datatypes import PromptInput
-        from riffusion.spectrogram_converter import SpectrogramConverter
         from riffusion.spectrogram_image_converter import _conform_channels
-        from riffusion.spectrogram_params import SpectrogramParams
         from riffusion.util import audio_util, image_util
 
-        if params is None:
-            params = SpectrogramParams(min_frequency=0, max_frequency=10000, stereo=False)
+        params = DEFAULT_PARAMS if params is None else params
         if max_batch < 1:
             raise ValueError("max_batch must be at least 1")
         if track.frame_rate != params.sample_rate:
@@ -588,10 +564,7 @@ class RiffusionPipeline:
         frames = a2a.clip_frames(clip_duration_s, params.sample_rate, params.hop_length)
         width, height = a2a.stride_32_size(frames, params.num_frequencies)
         a2a.check_denoising_size(width, height, clip_duration_s)
-        if converter is None:
-            converter = SpectrogramConverter(params, device=self.device)
-        if converter.p != params:
-            raise ValueError("converter was built for other SpectrogramParams")
+        converter = self._converter(params, converter)
 
         clips = [_conform_channels(c, params.stereo) for c in a2a.slice_audio_into_clips(track, starts, clip_duration_s)]
         waves = np.stack([np.array([c.get_array_of_samples() for c in clip.split_to_mono()]) for clip in clips])
@@ -621,7 +594,7 @@ class RiffusionPipeline:
                 n_evals.append(out["n_unet_evals"])
             else:
                 latents = torch.cat(self.riffuse_batch(requests[lo:hi], None, moments=moments, output_type="latent"))
-            u8 = ops.vae_image_to_u8(self.vae.decode(latents).sample)
+            u8 = self._decode_u8(latents)
             back, _ = ops.resize_bicubic_u8(u8, Ws, Hs)
             angles = None if init_angles is None else init_angles[lo:hi]
             out_waves.append(self._u8_to_waveform(back, converter, params.stereo, angles))
@@ -652,7 +625,8 @@ class RiffusionPipeline:
             text_embeddings=text_embeddings, init_latents=init_latents, generator_a=None, generator_b=None,
             interpolate_alpha=0.0, strength_a=strength, strength_b=strength, num_inference_steps=num_inference_steps,
             guidance_scale=guidance_scale, uncond_embeddings=uncond_embeddings, noise=noise, output_type="latent")
-        u8, wave = self._latents_to_audio(out["latents"], converter, False, init_angles)
+        u8 = self._decode_u8(out["latents"])
+        wave = self._u8_to_waveform(u8, converter, False, init_angles)
         return dict(images=u8, waveform=wave[:, 0], latents=out["latents"], latents_unscaled=out["latents_unscaled"],
                     n_unet_evals=out["n_unet_evals"])
 
@@ -680,6 +654,11 @@ def _load_weights(folder: Path) -> T.Dict[str, torch.Tensor]:
         if f.exists():
             return torch.load(str(f), map_location="cpu", weights_only=True)
     raise FileNotFoundError(f"no diffusers weight file under {folder}")
+
+
+def _sample_latents(mean: torch.Tensor, logvar: torch.Tensor, generator: torch.Generator) -> torch.Tensor:
+    """0.18215 * a sample of the VAE posterior with these moments, its fp32 noise drawn from `generator` (:259-264)."""
+    return VAE_SCALE * _Posterior(mean, logvar).sample(generator=generator)
 
 
 def preprocess_image(image: Image.Image) -> torch.Tensor:

@@ -1,10 +1,9 @@
-"""PNDM (PLMS) scheduler for the denoising loop — host-side tables + one fused device step.
+"""The schedulers of the denoising loops — host-side tables + one fused device step each.
 
-Restates diffusers 0.9 `PNDMScheduler(skip_prk_steps=True, steps_offset=1, beta_schedule="scaled_linear",
-beta_start=0.00085, beta_end=0.012, set_alpha_to_one=False)` [memory; SURVEY Appendix B], i.e. the scheduler
-`RiffusionPipeline.interpolate_img2img` drives at riffusion/riffusion_pipeline.py:314,361-365,379,392-396,403,418.
-The scalar recurrences (alphas, timestep table, multistep weights) run on the host in fp32; the tensor update
-runs in one kernel fused with the classifier-free-guidance combine (`rf_cfg_pndm_step_f16`).
+`PNDMSchedulerB200` and `DPMSolverMultistepSchedulerB200` share `_ScaledLinearScheduler`: the checkpoint's ᾱ table, the
+img2img `add_noise` (`rf_axpby_f16`, with the optional inpainting mask blend) and the diffusers-style `step`.  Each keeps
+its own timestep table and multistep bookkeeping on the host; the tensor update runs in one kernel fused with the
+classifier-free-guidance combine.
 """
 from __future__ import annotations
 
@@ -17,18 +16,45 @@ import torch
 from riffusion import tc_ops as ops
 
 
-class PNDMSchedulerB200:
+class _ScaledLinearScheduler:
+    """What both schedulers share: the ᾱ table of the checkpoint's scaled_linear betas (fp32), identity input scaling,
+    the img2img `add_noise` and the diffusers-style `step`.  Subclasses provide `set_timesteps`, `plan` and
+    `step_cfg`."""
     order = 1
+    init_noise_sigma = 1.0
+
+    def __init__(self, num_train_timesteps: int, beta_start: float, beta_end: float):
+        betas = torch.linspace(beta_start ** 0.5, beta_end ** 0.5, num_train_timesteps, dtype=torch.float32) ** 2
+        self.alphas_cumprod = torch.cumprod(1.0 - betas, dim=0)
+        self.num_train_timesteps = num_train_timesteps
+
+    def scale_model_input(self, sample: torch.Tensor, timestep=None) -> torch.Tensor:
+        return sample
+
+    def add_noise(self, original: torch.Tensor, noise: torch.Tensor, timestep, mask=None, blend_with=None) -> torch.Tensor:
+        """sqrt(ab_t) original + sqrt(1 - ab_t) noise; with `mask`, that where the mask is 1 and `blend_with` where it is
+        0 (the inpainting blend of interpolate_img2img, :420-425)."""
+        a = float(self.alphas_cumprod[int(timestep)])
+        return ops.axpby(original.contiguous(), noise.contiguous(), a ** 0.5, (1.0 - a) ** 0.5, mask, blend_with)
+
+    def step(self, model_output: torch.Tensor, timestep, sample: torch.Tensor, **kwargs):
+        """diffusers-compatible signature: the model output is already guided."""
+        pair = torch.cat([model_output, model_output]).contiguous()     # eps_u == eps_t  =>  guided eps == eps
+        return types.SimpleNamespace(prev_sample=self.step_cfg(pair, 0.0, int(timestep), sample))
+
+
+class PNDMSchedulerB200(_ScaledLinearScheduler):
+    """PNDM (PLMS).  Restates diffusers 0.9 `PNDMScheduler(skip_prk_steps=True, steps_offset=1,
+    beta_schedule="scaled_linear", beta_start=0.00085, beta_end=0.012, set_alpha_to_one=False)` [memory; SURVEY
+    Appendix B], i.e. the scheduler `RiffusionPipeline.interpolate_img2img` drives at
+    riffusion/riffusion_pipeline.py:314,361-365,379,392-396,403,418.  The scalar recurrences (alphas, timestep table,
+    multistep weights) run on the host in fp32; the tensor update is `rf_cfg_pndm_step_f16`."""
 
     def __init__(self, num_train_timesteps: int = 1000, beta_start: float = 0.00085, beta_end: float = 0.012,
                  steps_offset: int = 1):
-        betas = torch.linspace(beta_start ** 0.5, beta_end ** 0.5, num_train_timesteps, dtype=torch.float32) ** 2
-        self.alphas_cumprod = torch.cumprod(1.0 - betas, dim=0)
+        super().__init__(num_train_timesteps, beta_start, beta_end)
         self.final_alpha_cumprod = self.alphas_cumprod[0]
-        self.num_train_timesteps = num_train_timesteps
         self.config = {"steps_offset": steps_offset, "num_train_timesteps": num_train_timesteps}
-        self.init_noise_sigma = 1.0
-        self.timesteps: T.Optional[torch.Tensor] = None
         self.set_timesteps(50)
 
     # -- schedule -------------------------------------------------------------------------------
@@ -42,9 +68,6 @@ class PNDMSchedulerB200:
         self.counter = 0
         self.cur_sample: T.Optional[torch.Tensor] = None
 
-    def scale_model_input(self, sample: torch.Tensor, timestep=None) -> torch.Tensor:
-        return sample
-
     def _alpha(self, t: int) -> float:
         return float(self.alphas_cumprod[t]) if t >= 0 else float(self.final_alpha_cumprod)
 
@@ -53,10 +76,6 @@ class PNDMSchedulerB200:
         b_t, b_p = 1.0 - a_t, 1.0 - a_p
         denom = a_t * b_p ** 0.5 + (a_t * b_t * a_p) ** 0.5
         return (a_p / a_t) ** 0.5, (a_p - a_t) / denom
-
-    def add_noise(self, original: torch.Tensor, noise: torch.Tensor, timestep, mask=None, blend_with=None) -> torch.Tensor:
-        a = float(self.alphas_cumprod[int(timestep)])
-        return ops.axpby(original.contiguous(), noise.contiguous(), a ** 0.5, (1.0 - a) ** 0.5, mask, blend_with)
 
     # -- one multistep update ------------------------------------------------------------------------
     def plan(self, timestep: int):
@@ -96,13 +115,8 @@ class PNDMSchedulerB200:
         self.counter += 1
         return prev
 
-    def step(self, model_output: torch.Tensor, timestep, sample: torch.Tensor, **kwargs):
-        """diffusers-compatible signature: the model output is already guided."""
-        pair = torch.cat([model_output, model_output]).contiguous()     # eps_u == eps_t  =>  guided eps == eps
-        return types.SimpleNamespace(prev_sample=self.step_cfg(pair, 0.0, int(timestep), sample))
 
-
-class DPMSolverMultistepSchedulerB200:
+class DPMSolverMultistepSchedulerB200(_ScaledLinearScheduler):
     """DPM-Solver++ (2M) — host-side tables + one fused device step.
 
     Restates diffusers' `DPMSolverMultistepScheduler` with its defaults (`solver_order=2`, `algorithm_type="dpmsolver++"`,
@@ -116,24 +130,19 @@ class DPMSolverMultistepSchedulerB200:
     when fewer than 15 steps are run.  The scalar bookkeeping runs on the host in fp64 (from the fp32 ab table); the
     tensor update is one kernel fused with the guidance combine (`rf_cfg_dpmpp_step_f16`).
     """
-    order = 1
 
     def __init__(self, num_train_timesteps: int = 1000, beta_start: float = 0.00085, beta_end: float = 0.012,
                  solver_order: int = 2, lower_order_final: bool = True):
         if solver_order not in (1, 2):
             raise ValueError("solver_order must be 1 or 2")
-        betas = torch.linspace(beta_start ** 0.5, beta_end ** 0.5, num_train_timesteps, dtype=torch.float32) ** 2
-        self.alphas_cumprod = torch.cumprod(1.0 - betas, dim=0)
+        super().__init__(num_train_timesteps, beta_start, beta_end)
         ab = self.alphas_cumprod.double().numpy()
         self.alpha_t = np.sqrt(ab)
         self.sigma_t = np.sqrt(1.0 - ab)
         self.lambda_t = np.log(self.alpha_t) - np.log(self.sigma_t)
-        self.num_train_timesteps = num_train_timesteps
         self.config = {"num_train_timesteps": num_train_timesteps, "solver_order": solver_order,
                        "algorithm_type": "dpmsolver++", "solver_type": "midpoint", "lower_order_final": lower_order_final,
                        "prediction_type": "epsilon"}
-        self.init_noise_sigma = 1.0
-        self.timesteps: T.Optional[torch.Tensor] = None
         self.set_timesteps(50)
 
     def set_timesteps(self, num_inference_steps: int, device=None) -> None:
@@ -142,14 +151,6 @@ class DPMSolverMultistepSchedulerB200:
         self.timesteps = torch.from_numpy(ts.copy().astype(np.int64))
         self.model_outputs: T.List[T.Optional[torch.Tensor]] = [None] * self.config["solver_order"]
         self.lower_order_nums = 0
-
-    def scale_model_input(self, sample: torch.Tensor, timestep=None) -> torch.Tensor:
-        return sample
-
-    def add_noise(self, original: torch.Tensor, noise: torch.Tensor, timestep) -> torch.Tensor:
-        """img2img start point sqrt(ab_t) x + sqrt(1 - ab_t) noise, with the coefficients PNDM's add_noise uses."""
-        a = float(self.alphas_cumprod[int(timestep)])
-        return ops.axpby(original.contiguous(), noise.contiguous(), a ** 0.5, (1.0 - a) ** 0.5)
 
     def plan(self, timestep: int):
         """Host bookkeeping of one step: (order, (alpha_s0, sigma_s0, c_x, c_0, c_1)) in fp64.  A loop that starts
@@ -180,11 +181,6 @@ class DPMSolverMultistepSchedulerB200:
         self.model_outputs = self.model_outputs[1:] + [x0]
         self.lower_order_nums = min(self.lower_order_nums + 1, self.config["solver_order"])
         return prev
-
-    def step(self, model_output: torch.Tensor, timestep, sample: torch.Tensor, **kwargs):
-        """diffusers-compatible signature: the model output is already guided."""
-        pair = torch.cat([model_output, model_output]).contiguous()     # eps_u == eps_t  =>  guided eps == eps
-        return types.SimpleNamespace(prev_sample=self.step_cfg(pair, 0.0, int(timestep), sample))
 
 
 SCHEDULERS = {"DPMSolverMultistepScheduler": DPMSolverMultistepSchedulerB200, "PNDMScheduler": PNDMSchedulerB200}

@@ -205,7 +205,7 @@ class _RecordingUNet:
         return types.SimpleNamespace(sample=out.to(torch.float16))
 
 
-def _pipe(monkeypatch):
+def _pipe(monkeypatch, scheduler=None):
     from test_text_to_audio_cpu import _fake_dpm_step, _fake_pndm_step
 
     from riffusion import tc_ops
@@ -222,7 +222,7 @@ def _pipe(monkeypatch):
     monkeypatch.setattr(tc_ops, "cfg_pndm_step", _fake_pndm_step)
     monkeypatch.setattr(tc_ops, "axpby", axpby)
     unet = _RecordingUNet()
-    pipe = RiffusionPipeline(vae=None, unet=unet, device="cpu")
+    pipe = RiffusionPipeline(vae=None, unet=unet, scheduler=scheduler, device="cpu")
     pipe.use_cuda_graph = False
     return pipe, unet
 
@@ -264,6 +264,60 @@ def test_img2img_control_flow_and_draws(monkeypatch):
     with pytest.raises(ValueError, match="DPMSolverMultistepScheduler, PNDMScheduler"):
         pipe.img2img("", None, moments=(mean, logvar), scheduler="LMSDiscreteScheduler", text_embeddings=text,
                      uncond_embeddings=uncond)
+
+
+def test_zero_step_edge_of_both_img2img_entry_points(monkeypatch):
+    """when the start rule leaves no timestep to run, interpolate_img2img returns the latents noised at
+    timesteps[-init_timestep] (PNDM at 1 step: t = 1; DPM-Solver++ at 25 steps and strength 0.02: init_timestep = 0, so
+    timesteps[0] = 999) and img2img returns the clean latents; neither evaluates the UNet"""
+    from riffusion.riffusion_pipeline import VAE_SCALE
+    from riffusion.scheduler_b200 import DPMSolverMultistepSchedulerB200, PNDMSchedulerB200
+
+    torch.manual_seed(6)
+    lat, noise = torch.randn(2, 4, 8, 8).half(), torch.randn(2, 4, 8, 8).half()
+    mean, logvar = torch.randn(2, 4, 8, 8).half(), (torch.randn(2, 4, 8, 8) * 0.5 - 2).half()
+    text, uncond = torch.randn(2, 77, 16).half(), torch.randn(1, 77, 16).half()
+    for sched, name, steps, strength, t_noise in ((PNDMSchedulerB200(), "PNDMScheduler", 1, 0.8, 1),
+                                                  (DPMSolverMultistepSchedulerB200(), "DPMSolverMultistepScheduler", 25,
+                                                   0.02, 999)):
+        pipe, unet = _pipe(monkeypatch, scheduler=sched)
+        out = pipe.interpolate_img2img(text_embeddings=text, init_latents=lat, generator_a=None, generator_b=None,
+                                       interpolate_alpha=0.0, strength_a=strength, strength_b=strength,
+                                       num_inference_steps=steps, guidance_scale=7.0, uncond_embeddings=uncond,
+                                       noise=noise, output_type="latent")
+        a = float(sched.alphas_cumprod[t_noise])
+        assert out["n_unet_evals"] == 0 and not unet.inputs, name
+        assert torch.equal(out["latents_unscaled"], (a ** 0.5 * lat.float() + (1 - a) ** 0.5 * noise.float()).half())
+        out = pipe.img2img("", None, strength=strength, num_inference_steps=steps, seed=9, scheduler=name,
+                           output_type="latent", text_embeddings=text, uncond_embeddings=uncond, moments=(mean, logvar))
+        assert out["n_unet_evals"] == 0 and not unet.inputs and out["t_start"] == steps, name
+        for i in range(2):
+            post = torch.randn((1, 4, 8, 8), generator=torch.Generator().manual_seed(9))
+            std = torch.exp(0.5 * torch.clamp(logvar[i:i + 1], -30.0, 20.0))
+            clean = VAE_SCALE * (mean[i:i + 1].float() + std.float() * post).half()
+            assert torch.equal(out["latents_unscaled"][i:i + 1], clean), name
+
+
+def test_mismatched_uncond_embeddings_rejected_before_the_unet(monkeypatch):
+    """2 uncond rows for 3 clips would concatenate into a 5-row context; txt2img, img2img and interpolate_img2img raise
+    ValueError before the UNet runs"""
+    pipe, unet = _pipe(monkeypatch)
+    torch.manual_seed(7)
+    text, uncond = torch.randn(3, 77, 16).half(), torch.randn(2, 77, 16).half()
+    lat, logvar = torch.randn(3, 4, 8, 8).half(), torch.zeros(3, 4, 8, 8).half()
+    runs = [
+        lambda: pipe.txt2img("", num_clips=3, num_inference_steps=5, width=64, height=64, output_type="latent",
+                             text_embeddings=text, uncond_embeddings=uncond),
+        lambda: pipe.img2img("", None, num_inference_steps=5, output_type="latent", text_embeddings=text,
+                             uncond_embeddings=uncond, moments=(lat, logvar)),
+        lambda: pipe.interpolate_img2img(text_embeddings=text, init_latents=lat, generator_a=None, generator_b=None,
+                                         interpolate_alpha=0.0, num_inference_steps=5, uncond_embeddings=uncond,
+                                         noise=torch.randn(3, 4, 8, 8).half(), output_type="latent"),
+    ]
+    for run in runs:
+        with pytest.raises(ValueError, match="uncond_embeddings hold 2 rows for 3 clips"):
+            run()
+        assert not unet.inputs
 
 
 # ----------------------------------------------------------------------------------------------- CLI
