@@ -308,6 +308,11 @@ int rf_cfg_dpmpp_step_f16(const void* eps_pair, long n, float guidance, const vo
 /* y = a*x + b*noise (scheduler.add_noise), optionally y = y*mask + z*(1-mask) (riffusion_pipeline.py:421-425) */
 int rf_axpby_f16(const void* x, const void* noise, float a, float b, const void* mask, const void* z, long n,
                  void* y, void* stream);
+/* Magic Mix layout blend: u = mix * x + (1 - mix) * (a * enc + b * noise).  x, enc and u fp16, noise fp32 (n elements
+ *   each), a / b the add_noise coefficients of the step's timestep.  fp32 math with explicit roundings and one fp16
+ *   rounding of u; mix = 1 returns x bit for bit, mix = 0 is the plain noising of enc. */
+int rf_magic_mix_f16(const void* x, const void* enc, const float* noise, float a, float b, float mix, long n, void* u,
+                     void* stream);
 
 #ifdef __cplusplus
 }

@@ -727,6 +727,25 @@ __global__ void k_axpby(const __half* __restrict__ x, const __half* __restrict__
     }
 }
 
+// Magic Mix layout blend: u = mix * x + (1 - mix) * (a * enc + b * noise), i.e. the current latents mixed with the
+// clean encoding noised to this step's timestep (scheduler.add_noise).  x and enc are fp16, noise is the fp32 draw, kept
+// unrounded; a, b and mix are fp32.  Every product and sum has an explicit rounding and u is rounded to fp16 once, so
+// contraction cannot change a bit.  mix = 1 stores x itself (signed zeros and all); mix = 0 is the plain noising.
+__global__ void k_magic_mix(const __half* __restrict__ x, const __half* __restrict__ enc,
+                            const float* __restrict__ noise, float a, float b, float mix, size_t n,
+                            __half* __restrict__ u) {
+    const float w = __fsub_rn(1.f, mix);
+    for (size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < n;
+         i += static_cast<size_t>(gridDim.x) * blockDim.x) {
+        if (w == 0.f) {
+            u[i] = x[i];
+            continue;
+        }
+        const float noised = __fmaf_rn(b, noise[i], __fmul_rn(a, __half2float(enc[i])));
+        u[i] = __float2half_rn(__fmaf_rn(mix, __half2float(x[i]), __fmul_rn(w, noised)));
+    }
+}
+
 // 1x1 convolution on tiny channel counts, NCHW: y[b][o][p] = bias[o] + sum_i w[o][i] * (in_scale * x[b][i][p])
 __global__ void k_conv1x1_small(const __half* __restrict__ x, const __half* __restrict__ w, const __half* __restrict__ bias,
                                 int B, int Cin, int Cout, size_t HW, float in_scale, __half* __restrict__ y) {
@@ -1079,5 +1098,15 @@ extern "C" int rf_axpby_f16(const void* x, const void* noise, float a, float b, 
         static_cast<const __half*>(x), static_cast<const __half*>(noise), a, b, static_cast<const __half*>(mask),
         static_cast<const __half*>(z), static_cast<size_t>(n), static_cast<__half*>(y));
     RF_CUDA_LAUNCH_CHECK("k_axpby");
+    return RF_OK;
+}
+
+extern "C" int rf_magic_mix_f16(const void* x, const void* enc, const float* noise, float a, float b, float mix, long n,
+                                void* u, void* stream) {
+    if (!x || !enc || !noise || !u || n <= 0) return rf_fail(RF_ERR_INVALID, "rf_magic_mix_f16: bad argument");
+    k_magic_mix<<<grid_for(static_cast<size_t>(n), 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+        static_cast<const __half*>(x), static_cast<const __half*>(enc), noise, a, b, mix, static_cast<size_t>(n),
+        static_cast<__half*>(u));
+    RF_CUDA_LAUNCH_CHECK("k_magic_mix");
     return RF_OK;
 }

@@ -15,7 +15,8 @@ the same names, flags and defaults (`COMMANDS`, what `build_parser()` builds by 
         [--image-dir clips] [--negative-prompt ...] [--seed 42] [--denoising 0.55] [--num-inference-steps 25]
         [--guidance 7.0] [--scheduler DPMSolverMultistepScheduler] [--start-time-s 0] [--duration-s 20]
         [--clip-duration-s 5] [--overlap-duration-s 0.2] [--prompt-b ... [--seed-b N] [--denoising-b X]]
-        [--max-batch 32] [--use-20k] [--checkpoint DIR] [--device cuda]
+        [--max-batch 32] [--use-20k] [--magic-mix [--kmin 0.3] [--kmax 0.5] [--mix-factor 0.5]] [--checkpoint DIR]
+        [--device cuda]
 
 `text-to-audio` loads a local diffusers-layout checkpoint directory; with `--num-clips N` > 1 clip i (seed + i) is
 written to out_<seed + i>.wav / .png.  The image carries the spectrogram parameters in its EXIF block, so
@@ -234,10 +235,12 @@ def audio_to_audio(*, audio: str, output: str, prompt: str, image_dir: str = "",
                    seed: int = 42, denoising: float = 0.55, num_inference_steps: int = 25, guidance: float = 7.0,
                    scheduler: str = "DPMSolverMultistepScheduler", start_time_s: float = 0.0, duration_s: float = 20.0,
                    clip_duration_s: float = 5.0, overlap_duration_s: float = 0.2, prompt_b: str = "", seed_b: int = -1,
-                   denoising_b: float = -1.0, max_batch: int = 32, use_20k: bool = False,
+                   denoising_b: float = -1.0, max_batch: int = 32, use_20k: bool = False, magic_mix: bool = False,
+                   kmin: float = 0.3, kmax: float = 0.5, mix_factor: float = 0.5,
                    checkpoint: str = "riffusion/riffusion-model-v1", device: str = "cuda"):
     """Riff a track with a text prompt (overlapping clips, img2img, crossfaded back together); with --prompt-b,
-    interpolate from --prompt to --prompt-b along the track (--seed-b / --denoising-b: -1 = same as the first end)."""
+    interpolate from --prompt to --prompt-b along the track (--seed-b / --denoising-b: -1 = same as the first end);
+    with --magic-mix, restyle each clip with Magic Mix, keeping its layout (--kmin, --kmax, --mix-factor)."""
     from riffusion.riffusion_pipeline import RiffusionPipeline
 
     params = _app_params(use_20k)
@@ -248,7 +251,8 @@ def audio_to_audio(*, audio: str, output: str, prompt: str, image_dir: str = "",
         overlap_duration_s=overlap_duration_s, negative_prompt=negative_prompt or None, seed=seed, denoising=denoising,
         num_inference_steps=num_inference_steps, guidance_scale=guidance, scheduler=scheduler,
         prompt_b=prompt_b or None, seed_b=None if seed_b < 0 else seed_b,
-        denoising_b=None if denoising_b < 0 else denoising_b, max_batch=max_batch)
+        denoising_b=None if denoising_b < 0 else denoising_b, max_batch=max_batch, magic_mix=magic_mix, kmin=kmin,
+        kmax=kmax, mix_factor=mix_factor)
     segment = out["segment"]
     segment.export(output, format=Path(output).suffix[1:])
     print(f"Wrote {output} ({segment.duration_seconds:.2f} seconds, {len(out['clip_start_times'])} clips)")

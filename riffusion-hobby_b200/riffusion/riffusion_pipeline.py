@@ -372,23 +372,30 @@ class RiffusionPipeline:
 
     def _denoise(self, sched, timesteps, latents: torch.Tensor, context: torch.Tensor, guidance_scale: float,
                  mask: T.Optional[torch.Tensor] = None, init: T.Optional[torch.Tensor] = None,
-                 noise: T.Optional[torch.Tensor] = None) -> T.Tuple[torch.Tensor, int]:
+                 noise: T.Optional[torch.Tensor] = None,
+                 layout: T.Optional[T.Tuple[float, torch.Tensor, torch.Tensor, int]] = None) -> T.Tuple[torch.Tensor, int]:
         """The CFG loop over `timesteps`: one UNet evaluation of [latents | latents] (a captured CUDA graph when enabled)
         and one fused guidance + scheduler step each.  With a `mask`, every step is followed by the inpainting blend of
         interpolate_img2img (:420-425): `init` noised with `noise` at that step's timestep where the mask is 1, the
-        stepped latents where it is 0.  Returns (latents, evaluations)."""
+        stepped latents where it is 0.  With `layout` = (mix_factor, enc, noise32, stop), steps 1 .. stop - 1 of the
+        loop are Magic Mix's layout phase: the UNet evaluates mix_factor * latents + (1 - mix_factor) * add_noise(enc,
+        noise32, t) (`tc_ops.magic_mix`) and the scheduler still steps the latents.  Returns (latents, evaluations)."""
         do_cfg = guidance_scale > 1.0
         ctx_cache: T.Dict[str, T.Any] = {}
         graphed = self._graphed_unet(latents.shape, context) if do_cfg else None
         if mask is not None:
             mask = mask.to(device=latents.device, dtype=latents.dtype).expand_as(latents).contiguous()
         n_evals = 0
-        for t in timesteps:
+        for j, t in enumerate(timesteps):
             t_int = int(t)
+            unet_in = latents
+            if layout is not None and 0 < j < layout[3]:
+                a = float(sched.alphas_cumprod[t_int])
+                unet_in = ops.magic_mix(latents, layout[1], layout[2], a ** 0.5, (1.0 - a) ** 0.5, layout[0])
             if graphed is not None:
-                eps_pair = graphed(latents, t_int)
+                eps_pair = graphed(unet_in, t_int)
             else:
-                model_in = torch.cat([latents] * 2) if do_cfg else latents
+                model_in = torch.cat([unet_in] * 2) if do_cfg else unet_in
                 eps_pair = self.unet(model_in, t_int, encoder_hidden_states=context, ctx_cache=ctx_cache).sample
             n_evals += 1
             if not do_cfg:
@@ -439,14 +446,7 @@ class RiffusionPipeline:
         sched = make_scheduler(scheduler)
         sched.set_timesteps(num_inference_steps)
         dev = self._device
-        if moments is None:
-            if not torch.is_tensor(images):
-                images = torch.cat([preprocess_image(im) for im in images])
-            images = images.to(device=dev, dtype=torch.float16)
-            if images.dim() != 4 or images.shape[1] != 3 or images.shape[2] % 64 or images.shape[3] % 64:
-                raise ValueError(f"images must be (B, 3, H, W) with H and W multiples of 64, got {tuple(images.shape)}")
-            moments = self.vae.encode_moments(images.contiguous())
-        mean, logvar = moments
+        mean, logvar = self._image_moments(images, moments)
         n = mean.shape[0]
         context = self._context(prompt, negative_prompt, n, guidance_scale > 1.0, text_embeddings, uncond_embeddings)
         lats, draws = [], []
@@ -466,6 +466,80 @@ class RiffusionPipeline:
         latents, n_evals = self._denoise(sched, timesteps, latents, context, guidance_scale)
         out = self._finish(latents, n_evals, output_type)
         out["t_start"] = t_start
+        return out
+
+    def _image_moments(self, images, moments: T.Optional[T.Tuple[torch.Tensor, torch.Tensor]]):
+        """`moments` when given, else the VAE (mean, logvar) of `images`: PIL images (preprocessed like
+        `preprocess_image`) or a (B, 3, H, W) fp16 tensor in [-1, 1], H and W multiples of 64."""
+        if moments is not None:
+            return moments
+        if not torch.is_tensor(images):
+            images = torch.cat([preprocess_image(im) for im in images])
+        images = images.to(device=self._device, dtype=torch.float16)
+        if images.dim() != 4 or images.shape[1] != 3 or images.shape[2] % 64 or images.shape[3] % 64:
+            raise ValueError(f"images must be (B, 3, H, W) with H and W multiples of 64, got {tuple(images.shape)}")
+        return self.vae.encode_moments(images.contiguous())
+
+    @staticmethod
+    def magic_mix_range(num_inference_steps: int, kmin: float, kmax: float) -> T.Tuple[int, int]:
+        """(t_max, t_min) of Magic Mix: n - int(kmax * n) and n - int(kmin * n), indices into scheduler.timesteps.  The
+        loop starts at timesteps[t_max]; steps t_max + 1 .. t_min - 1 are the layout phase."""
+        n = num_inference_steps
+        if int(kmax * n) < 1:
+            raise ValueError(f"kmax * num_inference_steps must be at least 1 (kmax {kmax}, {n} steps): no step would run")
+        if kmax > 1.0:
+            raise ValueError(f"kmax must be at most 1, got {kmax}")
+        return n - int(kmax * n), n - int(kmin * n)
+
+    @torch.no_grad()
+    def magic_mix(self, prompt: str, images: T.Union[None, torch.Tensor, T.Sequence[Image.Image]], *, kmin: float = 0.3,
+                  kmax: float = 0.5, mix_factor: float = 0.5, num_inference_steps: int = 25, guidance_scale: float = 7.0,
+                  seed: int = 42, scheduler: str = "DPMSolverMultistepScheduler", output_type: T.Optional[str] = "pil",
+                  text_embeddings: T.Optional[torch.Tensor] = None, uncond_embeddings: T.Optional[torch.Tensor] = None,
+                  noise: T.Optional[torch.Tensor] = None,
+                  moments: T.Optional[T.Tuple[torch.Tensor, torch.Tensor]] = None) -> T.Dict[str, T.Any]:
+        """Magic Mix (Liew et al. 2022): restyle images with a prompt while keeping their layout, as the reference app's
+        "Use Magic Mix" switch runs it (streamlit/util.py:302-350, diffusers' community `magic_mix` pipeline), for a
+        batch of images in one CFG loop.  The algorithm is restated from memory, not pinned against diffusers
+        (unpinned).
+
+        With n = num_inference_steps, T = scheduler.timesteps (n entries for DPM-Solver++, n + 1 for PNDM), t_max =
+        n - int(kmax * n) and t_min = n - int(kmin * n) (`magic_mix_range`; int(kmax * n) < 1 raises ValueError):
+        enc = 0.18215 * posterior sample, x = add_noise(enc, noise, T[t_max]), then for every i >= t_max one CFG UNet
+        evaluation of u and one scheduler step of x, where u = mix_factor * x + (1 - mix_factor) * add_noise(enc, noise,
+        T[i]) in the layout phase t_max < i < t_min and u = x otherwise (`tc_ops.magic_mix`).  kmin >= kmax leaves no
+        layout phase: img2img started at T[t_max].
+
+        `noise` is torch.randn((1, 4, h, w)) in fp32 from a CPU generator seeded with `seed`, the same for every image
+        (the community pipeline's torch.manual_seed(seed)), and stays fp32.  Image i draws its posterior noise from its
+        own CUDA generator seeded with `seed`, as in `img2img` (the community pipeline uses the global CUDA RNG).  The
+        unconditional context is embed_text(""): Magic Mix has no negative prompt.  `images`, `moments`,
+        `text_embeddings`, `uncond_embeddings`, `scheduler` and `output_type` work as in `img2img`; an injected `noise`
+        is (1 or B, 4, h, w).  Returns dict(images, latents (1/0.18215-scaled), latents_unscaled, n_unet_evals, t_max,
+        t_min); n_unet_evals = len(T) - t_max."""
+        t_max, t_min = self.magic_mix_range(num_inference_steps, kmin, kmax)
+        sched = make_scheduler(scheduler)
+        sched.set_timesteps(num_inference_steps)
+        dev = self._device
+        mean, logvar = self._image_moments(images, moments)
+        n = mean.shape[0]
+        context = self._context(prompt, None, n, guidance_scale > 1.0, text_embeddings, uncond_embeddings)
+        enc = torch.cat([_sample_latents(mean[i:i + 1], logvar[i:i + 1],
+                                         torch.Generator(device=self.device).manual_seed(seed)) for i in range(n)])
+        enc = enc.to(device=dev, dtype=torch.float16).contiguous()
+        if noise is None:
+            noise = torch.randn((1,) + tuple(enc.shape[1:]), generator=torch.Generator().manual_seed(seed))
+        noise = noise.to(device=dev, dtype=torch.float32)
+        if noise.dim() != 4 or noise.shape[0] not in (1, n) or noise.shape[1:] != enc.shape[1:]:
+            raise ValueError(f"noise must be (1 or {n}, {', '.join(map(str, enc.shape[1:]))}), got {tuple(noise.shape)}")
+        noise = noise.expand_as(enc).contiguous()
+        timesteps = sched.timesteps[t_max:]
+        a = float(sched.alphas_cumprod[int(timesteps[0])])
+        latents = ops.magic_mix(enc, enc, noise, a ** 0.5, (1.0 - a) ** 0.5, 0.0)           # mix 0: add_noise at T[t_max]
+        latents, n_evals = self._denoise(sched, timesteps, latents, context, guidance_scale,
+                                         layout=(mix_factor, enc, noise, t_min - t_max))
+        out = self._finish(latents, n_evals, output_type)
+        out["t_max"], out["t_min"] = t_max, t_min
         return out
 
     @torch.no_grad()
@@ -527,7 +601,8 @@ class RiffusionPipeline:
                        seed_b: T.Optional[int] = None, denoising_b: T.Optional[float] = None, max_batch: int = 32,
                        init_angles: T.Optional[torch.Tensor] = None, apply_filters: bool = True,
                        text_embeddings: T.Optional[torch.Tensor] = None,
-                       uncond_embeddings: T.Optional[torch.Tensor] = None, converter=None) -> T.Dict[str, T.Any]:
+                       uncond_embeddings: T.Optional[torch.Tensor] = None, converter=None, magic_mix: bool = False,
+                       kmin: float = 0.3, kmax: float = 0.5, mix_factor: float = 0.5) -> T.Dict[str, T.Any]:
         """Riff a whole track: the reference app's Audio to Audio task (streamlit/tasks/audio_to_audio.py:86-330).
 
         The track (an AudioSegment at params.sample_rate) is cut into overlapping clips (`audio_to_audio.clip_start_times`,
@@ -541,7 +616,9 @@ class RiffusionPipeline:
         of n is `riffuse_batch` of InferenceInput(alpha = linspace(0, 1, n)[i], start = (prompt, seed, denoising),
         end = (prompt_b, seed_b, denoising_b)) - PNDM, weighted prompts, no negative prompt.  `init_angles` (clips,
         channels, n_fft/2 + 1, frames) fixes Griffin-Lim's initial phases; `text_embeddings` / `uncond_embeddings`
-        replace the text encoder of the img2img mode.
+        replace the text encoder of the img2img and Magic Mix modes.  With `magic_mix` every batch runs `magic_mix`
+        (prompt, `kmin`, `kmax`, `mix_factor`, `seed`, `scheduler`; `denoising` is not used) in place of `img2img`; it
+        cannot be combined with `prompt_b` or a negative prompt (ValueError), as in the app.
 
         Returns dict(segment (the stitched AudioSegment), source_images and images ((clips, H, W, 3) uint8 device tensors
         before and after denoising), denoised_images (the decoded images at the 32-stride size), clip_start_times (s), waveform ((clips, channels, L) fp32, before normalisation),
@@ -554,6 +631,12 @@ class RiffusionPipeline:
         params = DEFAULT_PARAMS if params is None else params
         if max_batch < 1:
             raise ValueError("max_batch must be at least 1")
+        if magic_mix and prompt_b is not None:
+            raise ValueError("magic_mix cannot be combined with interpolation (prompt_b)")
+        if magic_mix and negative_prompt:
+            raise ValueError("magic_mix takes no negative prompt")
+        if magic_mix:
+            self.magic_mix_range(num_inference_steps, kmin, kmax)          # its ValueError before any device work
         if track.frame_rate != params.sample_rate:
             track = track.set_frame_rate(params.sample_rate)        # the app resamples (audio_to_audio.py:89-91)
         starts = a2a.clip_start_times(track.duration_seconds, start_time_s, duration_s, clip_duration_s,
@@ -586,10 +669,17 @@ class RiffusionPipeline:
             _, vae_in = ops.resize_bicubic_u8(src, width, height, want_f16=True)
             moments = self.vae.encode_moments(vae_in)
             if prompt_b is None:
-                out = self.img2img(prompt, None, strength=denoising, num_inference_steps=num_inference_steps,
-                                   guidance_scale=guidance_scale, negative_prompt=negative_prompt, seed=seed,
-                                   scheduler=scheduler, output_type="latent", text_embeddings=text_embeddings,
-                                   uncond_embeddings=uncond_embeddings, moments=moments)
+                if magic_mix:
+                    out = self.magic_mix(prompt, None, kmin=kmin, kmax=kmax, mix_factor=mix_factor,
+                                         num_inference_steps=num_inference_steps, guidance_scale=guidance_scale,
+                                         seed=seed, scheduler=scheduler, output_type="latent",
+                                         text_embeddings=text_embeddings, uncond_embeddings=uncond_embeddings,
+                                         moments=moments)
+                else:
+                    out = self.img2img(prompt, None, strength=denoising, num_inference_steps=num_inference_steps,
+                                       guidance_scale=guidance_scale, negative_prompt=negative_prompt, seed=seed,
+                                       scheduler=scheduler, output_type="latent", text_embeddings=text_embeddings,
+                                       uncond_embeddings=uncond_embeddings, moments=moments)
                 latents = out["latents"]
                 n_evals.append(out["n_unet_evals"])
             else:

@@ -305,6 +305,19 @@ def axpby(x, noise, a, b, mask=None, z=None):
     return y
 
 
+def magic_mix(x, enc, noise, a, b, mix):
+    """Magic Mix layout blend fp16(mix * x + (1 - mix) * (a * enc + b * noise)) in one launch.  x, enc: fp16; noise:
+    fp32 of the same shape, not rounded to fp16; a, b: the add_noise coefficients of the step's timestep."""
+    _f16(x, "x"), _f16(enc, "enc")
+    if not noise.is_cuda or noise.dtype != torch.float32:
+        raise _native.NativeError(f"noise must be a CUDA fp32 tensor (got {noise.dtype} on {noise.device})")
+    assert enc.shape == x.shape == noise.shape and x.is_contiguous() and enc.is_contiguous() and noise.is_contiguous()
+    u = torch.empty_like(x)
+    _native.call("rf_magic_mix_f16", x.device, x.data_ptr(), enc.data_ptr(), noise.data_ptr(), float(a), float(b),
+                 float(mix), x.numel(), u.data_ptr())
+    return u
+
+
 def conv1x1_small(x_nchw: torch.Tensor, w: torch.Tensor, bias: torch.Tensor, in_scale: float = 1.0) -> torch.Tensor:
     """(B, Cin<=8, H, W) NCHW -> (B, Cout<=8, H, W); w: (Cout, Cin) fp16."""
     _f16(x_nchw, "x")

@@ -15,6 +15,9 @@ shape is warmed up and its CUDA graph captured before a timed window.  The line 
               time (rf_tc_profile_*, the accounting bench.py uses)
   gpu         card name, power limit and the median SM clock sampled during the timed window
 
+With `--magic-mix` every clip is riffed with Magic Mix (`--kmin 0.3 --kmax 0.5 --mix-factor 0.5`, the app's values) in
+place of img2img; the line then names the mode and carries its parameters instead of the denoising strength.
+
 Nothing is written to the repository.
 """
 from __future__ import annotations
@@ -33,6 +36,12 @@ ROOT = Path(__file__).resolve().parents[1]
 def output_seconds(n_clips: int, clip_duration_s: float, overlap_duration_s: float) -> float:
     """length of the stitched track: n clips, n - 1 crossfades"""
     return n_clips * clip_duration_s - (n_clips - 1) * overlap_duration_s
+
+
+def magic_mix_evals(steps: int, kmax: float, scheduler: str) -> int:
+    """CFG UNet evaluations of one Magic Mix call: len(timesteps) - t_max, t_max = steps - int(kmax * steps); PNDM's
+    table has steps + 1 entries"""
+    return steps + (scheduler == "PNDMScheduler") - (steps - int(kmax * steps))
 
 
 def synthetic_track(seconds: float, seed: int = 0, rate: int = 44100):
@@ -64,6 +73,10 @@ def main() -> None:
     ap.add_argument("--denoising", type=float, default=0.55)
     ap.add_argument("--scheduler", default="DPMSolverMultistepScheduler", choices=["DPMSolverMultistepScheduler", "PNDMScheduler"])
     ap.add_argument("--reps", type=int, default=2, help="timed repetitions of the batched call")
+    ap.add_argument("--magic-mix", action="store_true", help="riff with Magic Mix instead of img2img")
+    ap.add_argument("--kmin", type=float, default=0.3)
+    ap.add_argument("--kmax", type=float, default=0.5)
+    ap.add_argument("--mix-factor", type=float, default=0.5)
     args = ap.parse_args()
     import torch
 
@@ -91,6 +104,8 @@ def main() -> None:
     track = synthetic_track(args.seconds)
     kw = dict(params=params, duration_s=args.seconds, denoising=args.denoising, num_inference_steps=args.steps,
               scheduler=args.scheduler, text_embeddings=text, uncond_embeddings=uncond, converter=conv)
+    if args.magic_mix:
+        kw.update(magic_mix=True, kmin=args.kmin, kmax=args.kmax, mix_factor=args.mix_factor)
 
     def run(max_batch: int):
         with contextlib.redirect_stdout(sys.stderr):         # the per-clip channel warnings; stdout is the JSON line
@@ -110,6 +125,9 @@ def main() -> None:
     secs = output_seconds(n, 5.0, 0.2)
     assert abs(out["segment"].duration_seconds - secs) < 0.01, (out["segment"].duration_seconds, secs)
     n_evals = out["n_unet_evals"][0]
+    if args.magic_mix:
+        want = magic_mix_evals(args.steps, args.kmax, args.scheduler)
+        assert n_evals == want, (n_evals, want)
     sampler = ClockSampler(0)
     sampler.start()
     s_batched = wall(args.max_batch, args.reps)
@@ -141,6 +159,10 @@ def main() -> None:
                    "text": "N(0,1) embeddings", "reps": args.reps},
         "gpu": gpu_info(), "clocks": clocks,
     }
+    if args.magic_mix:
+        line["metric"] = "audio-to-audio (Magic Mix) output seconds per second"
+        line["config"]["magic_mix"] = {"kmin": args.kmin, "kmax": args.kmax, "mix_factor": args.mix_factor}
+        del line["config"]["denoising"]
     print(json.dumps(line))
 
 
