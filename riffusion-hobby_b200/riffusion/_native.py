@@ -9,6 +9,7 @@ from __future__ import annotations
 import ctypes as C
 import os
 import threading
+import typing as T
 from pathlib import Path
 
 import numpy as np
@@ -191,8 +192,58 @@ def call(name: str, device: torch.device, *args) -> None:
         check(getattr(lib(), name)(*args, stream_ptr(device)))
 
 
+def is_device_tensor(t: torch.Tensor) -> bool:
+    """Whether the library can read `t` through its pointer: a tensor in CUDA device memory."""
+    return t.is_cuda
+
+
+class _Any:
+    """An extent `operand` accepts whatever it is: equal to every int, so a shape check stays one tuple comparison."""
+    __slots__ = ()
+
+    def __eq__(self, other):
+        return True
+
+    def __ne__(self, other):
+        return False
+
+    __hash__ = object.__hash__
+
+    def __repr__(self):
+        return "?"
+
+
+ANY = _Any()
+
+
+def operand(t: torch.Tensor, name: str, dtype, shape=None, device=None, layout: T.Optional[str] = "dense") -> torch.Tensor:
+    """`t`, unchanged, once it meets its contract as an operand of a library call.  The C-ABI takes raw pointers and
+    cannot see a tensor's shape, dtype or device, so this check is what keeps a kernel inside its buffers.
+
+    dtype: a dtype, or a tuple of accepted ones.  shape: the exact shape as a tuple; an `ANY` entry matches any extent.
+    device: the device of the call's other operands.  layout: "dense" (row-major contiguous), "rows" (unit stride
+    along the last dim; the library checks the pitches) or None (any strides: the caller copies the tensor itself).
+    Reads metadata only (no tensor op, allocation or synchronisation), so it is safe during CUDA-graph capture.
+    Raises NativeError for a tensor outside device memory or of another dtype, ValueError for a wrong shape, layout
+    or device."""
+    if not is_device_tensor(t):
+        raise NativeError(f"{name} must be a CUDA tensor (no CPU fallback); got device {t.device}")
+    if t.dtype != dtype and not (isinstance(dtype, tuple) and t.dtype in dtype):
+        raise NativeError(f"{name} must be a {dtype} tensor, got {t.dtype}")
+    if device is not None and t.device != device:
+        raise ValueError(f"{name} is on {t.device}, the call's other operands on {device}")
+    if shape is not None and t.shape != shape:
+        raise ValueError(f"{name} must have shape {shape}, got {tuple(t.shape)}")
+    if layout == "dense" and not t.is_contiguous():
+        raise ValueError(f"{name} must be contiguous, got strides {t.stride()}")
+    if layout == "rows" and t.dim() and t.stride(-1) != 1:
+        raise ValueError(f"{name} must have unit stride along its last dim, got strides {t.stride()}")
+    return t
+
+
 def require_cuda(t: torch.Tensor, name: str, dtype: torch.dtype) -> torch.Tensor:
-    if not t.is_cuda:
+    """`t` as a contiguous tensor of `dtype` (converted and copied as needed); it must already be on a CUDA device."""
+    if not is_device_tensor(t):
         raise NativeError(f"{name} must be a CUDA tensor (no CPU fallback); got device {t.device}")
     if t.dtype != dtype:
         t = t.to(dtype)

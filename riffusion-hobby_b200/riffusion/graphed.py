@@ -35,7 +35,8 @@ class GraphedUNet:
     def set_context(self, context: torch.Tensor) -> None:
         """Re-target the captured graph to another text context of the same shape: the graph reads the context only
         through the cached cross-attention K / V^T tensors, which are recomputed into the same storage."""
-        assert context.shape == self.ctx.shape
+        if context.shape != self.ctx.shape:
+            raise ValueError(f"the graph was captured for a {tuple(self.ctx.shape)} context, got {tuple(context.shape)}")
         self.ctx.copy_(context)
         for key, (k, vt) in self.cache.items():
             k_new, vt_new = self.unet._kv(key, self.ctx)

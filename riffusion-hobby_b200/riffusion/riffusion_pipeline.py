@@ -158,9 +158,11 @@ class RiffusionPipeline:
         (1/0.18215-scaled) instead of a PIL image."""
         if moments is None:
             images = [init_images] * len(inputs) if isinstance(init_images, Image.Image) else list(init_images)
-            assert len(images) == len(inputs)
-        else:
-            assert init_images is None and moments[0].shape[0] == len(inputs)
+            if len(images) != len(inputs):
+                raise ValueError(f"{len(images)} init images for {len(inputs)} requests")
+        elif init_images is not None or moments[0].shape[0] != len(inputs):
+            raise ValueError(f"moments replace init_images (pass None for them) and need one row per request "
+                             f"({len(inputs)}), got {moments[0].shape[0]}")
         embed = self.embed_text_weighted if use_reweighting else self.embed_text
         groups: T.Dict[T.Tuple, T.List[int]] = {}
         for i, inp in enumerate(inputs):
@@ -583,7 +585,7 @@ class RiffusionPipeline:
         """uint8 images (B, H, W, 3) -> mel amplitudes (B, channels, H, W) -> waveform (B, channels, L)."""
         from riffusion import _native
 
-        B, H, W, _ = u8.shape
+        B, H, W, _ = _native.operand(u8, "u8", torch.uint8, shape=(_native.ANY, _native.ANY, _native.ANY, 3)).shape
         mel = torch.empty((B, 2 if stereo else 1, H, W), dtype=torch.float32, device=u8.device)
         p = converter.p
         for i in range(B):

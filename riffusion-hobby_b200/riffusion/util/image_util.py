@@ -82,8 +82,7 @@ def spectrogram_from_image_device(
     else:
         rgb = image
     rgb = _native.require_cuda(rgb, "image", torch.uint8)
-    H, W, C = rgb.shape
-    assert C == 3
+    H, W, _ = _native.operand(rgb, "image", torch.uint8, shape=(_native.ANY, _native.ANY, 3)).shape
     out = torch.empty((2 if stereo else 1, H, W), dtype=torch.float32, device=rgb.device)
     _native.call("rf_image_to_mel", rgb.device, rgb.data_ptr(), H, W, int(stereo), float(power), float(max_value),
                  out.data_ptr())
@@ -96,7 +95,7 @@ def image_from_spectrogram_device(spectrogram: torch.Tensor, power: float = 0.25
     from riffusion import _native
 
     s = _native.require_cuda(spectrogram, "spectrogram", torch.float32)
-    C, H, W = s.shape
+    C, H, W = _native.operand(s, "spectrogram", torch.float32, shape=(_native.ANY,) * 3).shape
     if C not in (1, 2):
         raise NotImplementedError(f"Unsupported number of channels: {C}")
     img = torch.empty((H, W, 3), dtype=torch.uint8, device=s.device)
