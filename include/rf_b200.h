@@ -297,6 +297,24 @@ int rf_slerp_f16(const void* v0, const void* v1, int B, long n, const float* d_a
 int rf_cfg_pndm_step_f16(const void* eps_pair, long n, float guidance, const void* h1, const void* h2,
                          const void* h3, const float* coef4, const void* sample, float ca, float cb,
                          void* eps_out, void* prev_sample, void* stream);
+/* One step of B independent PLMS loops, each row with its own multistep state and guidance.  The record of row r for
+ * this step (a DEVICE array of B records, one step's slice of a table uploaded before the loop):
+ *   active      0: prev = sample, bit for bit, and nothing else is written
+ *   guidance    g_r of eps = eps_u + g_r (eps_t - eps_u)
+ *   c0..c3      e = c0 eps + c1 ring[h1] + c2 ring[h2] + c3 ring[h3], a term only when its slot is 0..3 (-1 = absent)
+ *   ca, cb      prev = ca * base - cb * e; base = saved (flags & RF_PNDM_ROW_BASE_SAVED) or sample
+ *   push        ring slot 0..3 that receives the guided eps (-1 = none)
+ *   flags       RF_PNDM_ROW_SAVE: saved = sample (the first step, which PLMS's second call restarts from)
+ * ring: fp16 [4][B][m], saved: fp16 [B][m], eps_pair: fp16 [2B][m] = [uncond | text], sample / prev: fp16 [B][m].
+ * The arithmetic is rf_cfg_pndm_step_f16's term for term: a table whose rows all hold one step gives its bits. */
+#define RF_PNDM_ROW_BASE_SAVED 1
+#define RF_PNDM_ROW_SAVE 2
+typedef struct rf_pndm_row {
+    float guidance, c0, c1, c2, c3, ca, cb;
+    int32_t active, h1, h2, h3, push, flags;
+} rf_pndm_row;
+int rf_cfg_pndm_rows_step_f16(const void* eps_pair, int B, long m, const rf_pndm_row* d_rows, void* ring, void* saved,
+                              const void* sample, void* prev_sample, void* stream);
 /* classifier-free guidance + DPM-Solver++ (2M, midpoint) update on n = elements of ONE batch half:
  *   eps = eps_u + g (eps_t - eps_u) (fp16, as rf_cfg_pndm_step_f16); x0 = (x - sigma_s0 eps) / alpha_s0;
  *   prev = c_x x + c_0 x0 + c_1 (x0 - m1), the last term only when m1 (the previous step's x0) is given.

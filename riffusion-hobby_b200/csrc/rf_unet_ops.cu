@@ -687,6 +687,42 @@ __global__ void k_cfg_pndm_step(const __half* __restrict__ eps_pair, size_t n, f
     }
 }
 
+// k_cfg_pndm_step for B rows that each run their own PLMS loop (prompt-interpolation walks, where every row starts at
+// its own timestep and keeps its own guidance).  blockIdx.y = row; the row's record is read once per thread.  Slots
+// outside 0..3 count as absent, so a malformed record cannot index outside the ring.  Each element's ring / saved
+// reads come before its writes in the same thread, so no slot aliasing can race.
+__global__ void k_cfg_pndm_rows_step(const __half* __restrict__ eps_pair, int B, size_t m,
+                                     const rf_pndm_row* __restrict__ rows, __half* ring, __half* saved,
+                                     const __half* __restrict__ sample, __half* __restrict__ prev_sample) {
+    const int r = blockIdx.y;
+    const rf_pndm_row rec = rows[r];
+    const size_t row0 = static_cast<size_t>(r) * m, plane = static_cast<size_t>(B) * m;
+    const bool has1 = static_cast<unsigned>(rec.h1) < 4u, has2 = static_cast<unsigned>(rec.h2) < 4u,
+               has3 = static_cast<unsigned>(rec.h3) < 4u, push = static_cast<unsigned>(rec.push) < 4u;
+    const bool from_saved = rec.flags & RF_PNDM_ROW_BASE_SAVED, save = rec.flags & RF_PNDM_ROW_SAVE;
+    for (size_t k = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x; k < m;
+         k += static_cast<size_t>(gridDim.x) * blockDim.x) {
+        const size_t i = row0 + k;
+        if (!rec.active) {
+            prev_sample[i] = sample[i];
+            continue;
+        }
+        const __half eu = eps_pair[i], et = eps_pair[plane + i];
+        const __half d = __hsub(et, eu);
+        const __half gd = __float2half_rn(__half2float(d) * rec.guidance);
+        const __half e0 = __hadd(eu, gd);
+        float e = __fmul_rn(rec.c0, __half2float(e0));
+        if (has1) e = __fmaf_rn(rec.c1, __half2float(ring[rec.h1 * plane + i]), e);
+        if (has2) e = __fmaf_rn(rec.c2, __half2float(ring[rec.h2 * plane + i]), e);
+        if (has3) e = __fmaf_rn(rec.c3, __half2float(ring[rec.h3 * plane + i]), e);
+        const __half x = sample[i];
+        const float base = __half2float(from_saved ? saved[i] : x);
+        if (push) ring[rec.push * plane + i] = e0;
+        if (save) saved[i] = x;
+        prev_sample[i] = __float2half_rn(__fmaf_rn(rec.ca, base, -__fmul_rn(rec.cb, e)));
+    }
+}
+
 // eps = eps_u + g (eps_t - eps_u)               fp16 arithmetic, bit-identical to k_cfg_pndm_step's
 // x0  = (x - sigma_s0 eps) / alpha_s0           DPMSolverMultistepScheduler.convert_model_output ("dpmsolver++")
 // x'  = c_x x + c_0 x0 + c_1 (x0 - m1)          first order (m1 == NULL) or the 2M midpoint update
@@ -1075,6 +1111,20 @@ extern "C" int rf_cfg_pndm_step_f16(const void* eps_pair, long n, float guidance
         static_cast<const __half*>(h2), static_cast<const __half*>(h3), coef4[0], coef4[1], coef4[2], coef4[3],
         static_cast<const __half*>(sample), ca, cb, static_cast<__half*>(eps_out), static_cast<__half*>(prev_sample));
     RF_CUDA_LAUNCH_CHECK("k_cfg_pndm_step");
+    return RF_OK;
+}
+
+extern "C" int rf_cfg_pndm_rows_step_f16(const void* eps_pair, int B, long m, const rf_pndm_row* d_rows, void* ring,
+                                         void* saved, const void* sample, void* prev_sample, void* stream) {
+    if (!eps_pair || !d_rows || !ring || !saved || !sample || !prev_sample || B <= 0 || B > 65535 || m <= 0)
+        return rf_fail(RF_ERR_INVALID, "rf_cfg_pndm_rows_step_f16: bad argument");
+    const size_t per_row = static_cast<size_t>(m);
+    // the grid-stride budget of the whole batch, split evenly over the rows
+    const unsigned bx = std::max(1u, grid_for(per_row * B, 256) / static_cast<unsigned>(B));
+    k_cfg_pndm_rows_step<<<dim3(bx, static_cast<unsigned>(B)), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+        static_cast<const __half*>(eps_pair), B, per_row, d_rows, static_cast<__half*>(ring),
+        static_cast<__half*>(saved), static_cast<const __half*>(sample), static_cast<__half*>(prev_sample));
+    RF_CUDA_LAUNCH_CHECK("k_cfg_pndm_rows_step");
     return RF_OK;
 }
 

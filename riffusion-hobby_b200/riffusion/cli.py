@@ -17,6 +17,10 @@ the same names, flags and defaults (`COMMANDS`, what `build_parser()` builds by 
         [--clip-duration-s 5] [--overlap-duration-s 0.2] [--prompt-b ... [--seed-b N] [--denoising-b X]]
         [--max-batch 32] [--use-20k] [--magic-mix [--kmin 0.3] [--kmax 0.5] [--mix-factor 0.5]] [--checkpoint DIR]
         [--device cuda]
+    python -m riffusion.cli interpolation --prompt-a "jazz" --prompt-b "rock" --seed-image og_beat.png --output walk.wav
+        [--image-dir steps] [--seed-a 42] [--seed-b 42] [--denoising-a 0.75] [--denoising-b 0.75] [--guidance 7.0]
+        [--num-interpolation-steps 12] [--num-inference-steps 50] [--alpha-power 1.0] [--max-batch 32]
+        [--checkpoint DIR] [--device cuda]
 
 `text-to-audio` loads a local diffusers-layout checkpoint directory; with `--num-clips N` > 1 clip i (seed + i) is
 written to out_<seed + i>.wav / .png.  The image carries the spectrogram parameters in its EXIF block, so
@@ -266,11 +270,37 @@ def audio_to_audio(*, audio: str, output: str, prompt: str, image_dir: str = "",
         print(f"Wrote {2 * len(images)} images to {image_dir}")
 
 
+def interpolation(*, prompt_a: str, prompt_b: str, seed_image: str, output: str, image_dir: str = "", seed_a: int = 42,
+                  seed_b: int = 42, denoising_a: float = 0.75, denoising_b: float = 0.75, guidance: float = 7.0,
+                  num_interpolation_steps: int = 12, num_inference_steps: int = 50, alpha_power: float = 1.0,
+                  max_batch: int = 32, checkpoint: str = "riffusion/riffusion-model-v1", device: str = "cuda"):
+    """Walk from --prompt-a (--seed-a, --denoising-a) to --prompt-b (--seed-b, --denoising-b) on a seed spectrogram
+    image in --num-interpolation-steps clips, appended into one track (--alpha-power shapes the walk)."""
+    from riffusion.datatypes import PromptInput
+    from riffusion.riffusion_pipeline import DEFAULT_PARAMS, RiffusionPipeline
+
+    start = PromptInput(prompt=prompt_a, seed=seed_a, denoising=denoising_a, guidance=guidance)
+    end = PromptInput(prompt=prompt_b, seed=seed_b, denoising=denoising_b, guidance=guidance)
+    init_image = Image.open(seed_image).convert("RGB")
+    pipe = RiffusionPipeline.load_checkpoint(checkpoint=checkpoint, device=device)
+    out = pipe.interpolation(start, end, init_image, num_interpolation_steps=num_interpolation_steps,
+                             num_inference_steps=num_inference_steps, alpha_power=alpha_power, max_batch=max_batch)
+    segment = out["segment"]
+    segment.export(output, format=Path(output).suffix[1:])
+    print(f"Wrote {output} ({segment.duration_seconds:.2f} seconds, {len(out['alphas'])} steps)")
+    if image_dir:
+        target = Path(image_dir)
+        target.mkdir(parents=True, exist_ok=True)
+        for i, im in enumerate(out["images"].cpu().numpy()):
+            _store_spectrogram(im, DEFAULT_PARAMS, target / f"step_{i}.png")
+        print(f"Wrote {len(out['alphas'])} images to {image_dir}")
+
+
 COMMANDS = [audio_to_image, image_to_audio, sample_clips, print_exif, audio_to_images_batch, sample_clips_batch]
 # commands of this package that the reference's CLI does not have; `main` offers them next to COMMANDS
 EXTRA_COMMANDS = [text_to_audio]
-# the track-level command, offered by `main` after EXTRA_COMMANDS
-TRACK_COMMANDS = [audio_to_audio]
+# the track-level commands, offered by `main` after EXTRA_COMMANDS
+TRACK_COMMANDS = [audio_to_audio, interpolation]
 
 
 # ------------------------------------------------------------------------------------------------ argparse front end

@@ -178,34 +178,124 @@ class RiffusionPipeline:
             mask = preprocess_mask(mask_image, scale_factor=vae_scale_factor).to(device=self.device, dtype=torch.float16)
         results: T.List[T.Optional[Image.Image]] = [None] * len(inputs)
         for (strength, guidance, steps), idx in groups.items():
-            texts, lats, nas, nbs, alphas = [], [], [], [], []
-            for i in idx:
-                inp = inputs[i]
-                e0, e1 = embed(inp.start.prompt), embed(inp.end.prompt)
-                texts.append(e0 + inp.alpha * (e1 - e0))
-                g_post = torch.Generator(device=self.device).manual_seed(inp.start.seed)
-                if moments is None:
-                    lats.append(self.encode_image(images[i], g_post))
-                else:
-                    lats.append(_sample_latents(moments[0][i:i + 1], moments[1][i:i + 1], g_post))
-                ga = torch.Generator(device=self.device).manual_seed(inp.start.seed)
-                gb = torch.Generator(device=self.device).manual_seed(inp.end.seed)
-                shape = lats[-1].shape
-                nas.append(torch.randn(shape, generator=ga, device=self.device, dtype=torch.float16))
-                nbs.append(torch.randn(shape, generator=gb, device=self.device, dtype=torch.float16))
-                alphas.append(float(inp.alpha))
-            na, nb = torch.cat(nas), torch.cat(nbs)
-            if self.device_slerp:
-                noise = ops.slerp(alphas, na, nb)
-            else:
-                noise = torch.cat([torch_util.slerp(al, na[j:j + 1], nb[j:j + 1]) for j, al in enumerate(alphas)])
+            texts, lats, noise = self._prepare_requests(inputs, idx, embed, images if moments is None else None, moments)
             out = self.interpolate_img2img(
-                text_embeddings=torch.cat(texts), init_latents=torch.cat(lats), mask=mask, generator_a=None, generator_b=None,
+                text_embeddings=texts, init_latents=lats, mask=mask, generator_a=None, generator_b=None,
                 interpolate_alpha=0.0, strength_a=strength, strength_b=strength, num_inference_steps=steps,
                 guidance_scale=guidance, noise=noise, output_type=output_type)
             for j, i in enumerate(idx):
                 results[i] = out["latents"][j:j + 1] if output_type == "latent" else out["images"][j]
         return results  # type: ignore[return-value]
+
+    def _prepare_requests(self, inputs: T.Sequence[InferenceInput], idx: T.Sequence[int], embed,
+                          images: T.Optional[T.Sequence[Image.Image]],
+                          moments: T.Optional[T.Tuple[torch.Tensor, torch.Tensor]]):
+        """What `riffuse` draws for each request inputs[i], i in idx: the prompt embeddings lerped at the request's
+        alpha, the VAE posterior sample of images[i] (or of row i of `moments`) and noise_a from a generator seeded with
+        start.seed, noise_b from one seeded with end.seed, and their slerp at alpha.  Returns (text embeddings, latents,
+        noise), one row per request in idx order."""
+        texts, lats, nas, nbs, alphas = [], [], [], [], []
+        for i in idx:
+            inp = inputs[i]
+            e0, e1 = embed(inp.start.prompt), embed(inp.end.prompt)
+            texts.append(e0 + inp.alpha * (e1 - e0))
+            g_post = torch.Generator(device=self.device).manual_seed(inp.start.seed)
+            if moments is None:
+                lats.append(self.encode_image(images[i], g_post))
+            else:
+                lats.append(_sample_latents(moments[0][i:i + 1], moments[1][i:i + 1], g_post))
+            ga = torch.Generator(device=self.device).manual_seed(inp.start.seed)
+            gb = torch.Generator(device=self.device).manual_seed(inp.end.seed)
+            shape = lats[-1].shape
+            nas.append(torch.randn(shape, generator=ga, device=self.device, dtype=torch.float16))
+            nbs.append(torch.randn(shape, generator=gb, device=self.device, dtype=torch.float16))
+            alphas.append(float(inp.alpha))
+        na, nb = torch.cat(nas), torch.cat(nbs)
+        if self.device_slerp:
+            noise = ops.slerp(alphas, na, nb)
+        else:
+            noise = torch.cat([torch_util.slerp(al, na[j:j + 1], nb[j:j + 1]) for j, al in enumerate(alphas)])
+        return torch.cat(texts), torch.cat(lats), noise
+
+    # ------------------------------------------------------------------------------ interpolation
+    @staticmethod
+    def interpolation_alphas(n: int, p: float = 1.0) -> np.ndarray:
+        """The alphas of the app's interpolation task (streamlit/tasks/interpolation.py:99-104): linspace(0, 1, n) mapped
+        through x = 2a - 1, a' = (|x|^p sign(x) + 1) / 2, so p > 1 packs the alphas towards 0.5 and p < 1 towards the two ends."""
+        a = np.linspace(0, 1, n) * 2 - 1
+        return (np.abs(a) ** p * np.sign(a) + 1) / 2
+
+    @torch.no_grad()
+    def interpolation(self, start, end, init_image: Image.Image, *, num_interpolation_steps: int = 12,
+                      num_inference_steps: int = 50, alpha_power: float = 1.0, params=None, max_batch: int = 32,
+                      init_angles: T.Optional[torch.Tensor] = None, apply_filters: bool = True) -> T.Dict[str, T.Any]:
+        """A track that walks from `start` to `end` (PromptInputs: prompt, seed, denoising, guidance) on `init_image`:
+        the app's Interpolation task (streamlit/tasks/interpolation.py:99-181).  Clip i is `riffuse` of
+        InferenceInput(alpha_i, num_inference_steps, start, end) with alpha_i = interpolation_alphas(n, alpha_power)[i]
+        (PNDM, weighted prompts, no negative prompt, no mask), turned into audio with `params` (default mono 0-10 kHz)
+        and appended to the previous clips without a crossfade.
+
+        Every row draws what `riffuse` draws for its request (`_prepare_requests`) and is noised at its own start
+        timestep; then up to `max_batch` rows run as one CFG loop (`PNDMRowsB200`): each row joins at its own
+        `_img2img_steps` start and keeps its own guidance, so a walk whose ends differ in denoising or guidance still
+        runs as one loop.  After the loop, on the device: VAE decode -> uint8 image -> mel -> waveform
+        (`init_angles` (n, channels, n_fft/2 + 1, frames) fixes Griffin-Lim's initial phases); on the host:
+        peak-normalised int16, `apply_filters`, `stitch_segments` with no crossfade.  The page round-trips each clip
+        through MP3 bytes before joining; here the clips are joined as int16 PCM.
+
+        Raises ValueError before any device work when num_interpolation_steps or max_batch is below 1, when the two
+        ends' guidance lies on different sides of 1, or when the seed image's height (rounded down to a multiple of 32)
+        is not params.num_frequencies.  Returns dict(segment, images ((n, H, W, 3) uint8 device
+        tensor), waveform ((n, channels, L) fp32 before normalisation), alphas, requests, n_unet_evals (per loop))."""
+        from riffusion.scheduler_b200 import PNDMRowsB200
+        from riffusion.util import audio_util
+
+        n = num_interpolation_steps
+        if n < 1:
+            raise ValueError("num_interpolation_steps must be at least 1")
+        if max_batch < 1:
+            raise ValueError("max_batch must be at least 1")
+        if (start.guidance > 1.0) != (end.guidance > 1.0):
+            raise ValueError(f"the guidance of the two ends ({start.guidance}, {end.guidance}) lies on different sides "
+                             "of 1: only some clips would use classifier-free guidance")
+        params = DEFAULT_PARAMS if params is None else params
+        if init_image.height - init_image.height % 32 != params.num_frequencies:
+            raise ValueError(f"the seed image is {init_image.height} pixels high; params.num_frequencies "
+                             f"{params.num_frequencies} needs that height (rounded down to a multiple of 32)")
+        alphas = self.interpolation_alphas(n, alpha_power)
+        requests = [InferenceInput(start=start, end=end, alpha=float(a), num_inference_steps=num_inference_steps)
+                    for a in alphas]
+        sched = PNDMSchedulerB200()
+        sched.set_timesteps(num_inference_steps)
+        strengths = [(1 - r.alpha) * start.denoising + r.alpha * end.denoising for r in requests]   # as riffuse
+        guidances = [start.guidance * (1.0 - r.alpha) + end.guidance * r.alpha for r in requests]
+        steps = [self._img2img_steps(sched, num_inference_steps, s) for s in strengths]
+        converter = self._converter(params, None)
+        images = [init_image] * n
+        u8s, waves, n_evals = [], [], []
+        for lo in range(0, n, max_batch):
+            idx = list(range(lo, min(n, lo + max_batch)))
+            texts, lats, noise = self._prepare_requests(requests, idx, self.embed_text_weighted, images, None)
+            lats = lats.to(device=self._device, dtype=torch.float16).contiguous()
+            noise = noise.to(self._device, torch.float16).contiguous()
+            latents = torch.cat([sched.add_noise(lats[j:j + 1], noise[j:j + 1], int(sched.timesteps[-steps[i][0]]))
+                                 for j, i in enumerate(idx)])
+            rows = PNDMRowsB200(num_inference_steps, [steps[i][1] for i in idx], [guidances[i] for i in idx],
+                                device=self._device)
+            context = self._context(None, None, len(idx), guidances[lo] > 1.0, texts, None)
+            latents, evals = self._denoise(rows, rows.timesteps, latents, context, guidances[lo])
+            n_evals.append(evals)
+            u8 = self._decode_u8((1.0 / VAE_SCALE) * latents)
+            angles = None if init_angles is None else init_angles[lo:lo + len(idx)]
+            waves.append(self._u8_to_waveform(u8, converter, params.stereo, angles))
+            u8s.append(u8)
+        waveform = torch.cat(waves)
+        segments = []
+        for w in waveform.cpu().numpy():
+            seg = audio_util.audio_from_waveform(samples=w, sample_rate=params.sample_rate, normalize=True)
+            segments.append(audio_util.apply_filters(seg, compression=False) if apply_filters else seg)
+        return dict(segment=audio_util.stitch_segments(segments, crossfade_s=0), images=torch.cat(u8s),
+                    waveform=waveform, alphas=alphas, requests=requests, n_unet_evals=n_evals)
 
     def encode_image(self, init_image: Image.Image, generator: torch.Generator) -> torch.Tensor:
         """preprocess + VAE posterior sample * 0.18215 (:252-264).  The (mean, logvar) moments only depend on the

@@ -13,7 +13,9 @@ import typing as T
 import numpy as np
 import torch
 
+from riffusion import _native
 from riffusion import tc_ops as ops
+from riffusion._native import operand
 
 
 class _ScaledLinearScheduler:
@@ -104,15 +106,117 @@ class PNDMSchedulerB200(_ScaledLinearScheduler):
         """Guidance combine (riffusion_pipeline.py:411-415) + scheduler.step (:418) in one kernel.
         eps_pair = UNet output for [uncond | text]."""
         coef, hist, override, push, ca, cb = self.plan(timestep)
-        if self.counter == 0:
-            self.cur_sample = sample
         base = sample if override is None else override
         eps, prev = ops.cfg_pndm_step(eps_pair.contiguous(), guidance, hist, coef, base.contiguous(), ca, cb, want_eps=push)
+        self.advance(sample, eps, push, override)
+        return prev
+
+    def advance(self, sample, eps, push: bool, override) -> None:
+        """The multistep bookkeeping after the step `plan` described: the first step's sample is kept for the second
+        call's restart, a pushed eps joins the history (the last 4 are kept), the restart releases the kept sample.
+        `sample` and `eps` are only stored, never read, so `PNDMRowsB200` runs this with slot tokens."""
+        if self.counter == 0:
+            self.cur_sample = sample
         if push:
             self.ets = self.ets[-3:] + [eps]
         elif override is not None:
             self.cur_sample = None
         self.counter += 1
+
+
+ROW_DTYPE = np.dtype([(name, np.float32) for name in ("guidance", "c0", "c1", "c2", "c3", "ca", "cb")] +
+                     [(name, np.int32) for name in ("active", "h1", "h2", "h3", "push", "flags")])   # rf_pndm_row
+ROW_BASE_SAVED, ROW_SAVE = 1, 2           # RF_PNDM_ROW_BASE_SAVED, RF_PNDM_ROW_SAVE
+_SAVED = "saved"                          # the token `advance` keeps as a row's first sample
+
+
+def cfg_pndm_rows_step(eps_pair: torch.Tensor, rows: torch.Tensor, ring: torch.Tensor, saved: torch.Tensor,
+                       sample: torch.Tensor) -> torch.Tensor:
+    """One PLMS step of B rows with per-row state (`rf_cfg_pndm_rows_step_f16`).  eps_pair: (2B, ...) fp16 [uncond |
+    text]; rows: (B, 13) int32, this step's `ROW_DTYPE` records; ring: (4, B, ...) fp16 eps history, updated in place;
+    saved: (B, ...) fp16, the rows' first samples, updated in place; sample: (B, ...) fp16.  Returns prev_sample."""
+    operand(sample, "sample", torch.float16)
+    dev = sample.device
+    if sample.dim() < 1 or sample.numel() == 0:
+        raise ValueError(f"sample must hold at least one element per row, got shape {tuple(sample.shape)}")
+    B = sample.shape[0]
+    operand(eps_pair, "eps_pair", torch.float16, shape=(2 * B, *sample.shape[1:]), device=dev)
+    operand(rows, "rows", torch.int32, shape=(B, ROW_DTYPE.itemsize // 4), device=dev)
+    operand(ring, "ring", torch.float16, shape=(4, *sample.shape), device=dev)
+    operand(saved, "saved", torch.float16, shape=sample.shape, device=dev)
+    prev = torch.empty_like(sample)
+    _native.call("rf_cfg_pndm_rows_step_f16", dev, eps_pair.data_ptr(), B, sample.numel() // B, rows.data_ptr(),
+                 ring.data_ptr(), saved.data_ptr(), sample.data_ptr(), prev.data_ptr())
+    return prev
+
+
+class PNDMRowsB200:
+    """B independent PNDM img2img loops run as one: row r runs `PNDMSchedulerB200`'s steps over timesteps[t_starts[r]:]
+    with guidance guidances[r], and all rows end on the same last timestep.  `RiffusionPipeline._denoise` drives it in
+    place of a scheduler over `timesteps` = timesteps[min(t_starts):]; a row whose start has not come yet is carried
+    through unchanged.
+
+    The whole (steps x rows) table of `ROW_DTYPE` records is derived before the loop from one `PNDMSchedulerB200` per
+    row (its `plan` and `advance`, run with ring-slot tokens in place of tensors) and uploaded once; each `step_cfg` is
+    one `rf_cfg_pndm_rows_step_f16` launch on that step's slice.  The eps history is a 4-slot ring per row: PLMS keeps
+    at most 4 eps and a step reads at most 3 while writing 1.  Rows all on one side of guidance 1: above it the table
+    holds each row's guidance, otherwise 0 (the loop then passes [eps | eps]).  `t_starts[r] == len(timesteps)` is a
+    row that never runs a step."""
+
+    def __init__(self, num_inference_steps: int, t_starts: T.Sequence[int], guidances: T.Sequence[float],
+                 device="cuda"):
+        if len(t_starts) != len(guidances) or not len(t_starts):
+            raise ValueError(f"need one t_start and one guidance per row, got {len(t_starts)} and {len(guidances)}")
+        cfg = {float(g) > 1.0 for g in guidances}
+        if len(cfg) != 1:
+            raise ValueError("the rows' guidance lies on both sides of 1: only some rows would use guidance")
+        use_cfg = cfg.pop()
+        ref = PNDMSchedulerB200()
+        ref.set_timesteps(num_inference_steps)
+        self.all_timesteps = ref.timesteps
+        n_t = len(self.all_timesteps)
+        if any(not 0 <= int(t) <= n_t for t in t_starts):
+            raise ValueError(f"t_starts must lie in 0..{n_t}, got {list(t_starts)}")
+        self.t0 = min(int(t) for t in t_starts)
+        self.timesteps = self.all_timesteps[self.t0:]
+        table = np.zeros((n_t - self.t0, len(t_starts)), dtype=ROW_DTYPE)
+        for name in ("h1", "h2", "h3", "push"):
+            table[name] = -1
+        for r, (t_start, g) in enumerate(zip(t_starts, guidances)):
+            s = PNDMSchedulerB200()
+            s.set_timesteps(num_inference_steps)
+            pushes = 0
+            for i in range(int(t_start), n_t):
+                coef, hist, override, push, ca, cb = s.plan(int(self.all_timesteps[i]))
+                rec = table[i - self.t0, r]
+                rec["active"] = 1
+                rec["guidance"] = float(g) if use_cfg else 0.0
+                rec["c0"], rec["c1"], rec["c2"], rec["c3"] = coef
+                rec["ca"], rec["cb"] = ca, cb
+                for name, slot in zip(("h1", "h2", "h3"), hist):
+                    rec[name] = slot
+                slot = pushes % 4 if push else -1
+                rec["push"] = slot
+                rec["flags"] = (ROW_SAVE if s.counter == 0 else 0) | (ROW_BASE_SAVED if override == _SAVED else 0)
+                s.advance(_SAVED, slot, push, override)
+                pushes += push
+        self.table = table
+        self.rows = torch.from_numpy(table.view(np.int32).reshape(table.shape + (ROW_DTYPE.itemsize // 4,))).to(device)
+        self.ring: T.Optional[torch.Tensor] = None
+        self.saved: T.Optional[torch.Tensor] = None
+        self.step_index = 0
+
+    def step_cfg(self, eps_pair: torch.Tensor, guidance: float, timestep: int, sample: torch.Tensor) -> torch.Tensor:
+        """Guidance combine + every row's PLMS step for the next timestep of the table in one kernel.  The guidance
+        scalar of the loop is not used: each row's is in the table."""
+        j = self.step_index
+        if j >= len(self.timesteps) or int(timestep) != int(self.timesteps[j]):
+            raise ValueError(f"step {j} of this table is not timestep {int(timestep)}")
+        if self.ring is None:
+            self.ring = torch.empty((4, *sample.shape), dtype=sample.dtype, device=sample.device)
+            self.saved = torch.empty_like(sample)
+        prev = cfg_pndm_rows_step(eps_pair.contiguous(), self.rows[j], self.ring, self.saved, sample.contiguous())
+        self.step_index += 1
         return prev
 
 
