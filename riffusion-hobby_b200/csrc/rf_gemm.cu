@@ -552,7 +552,8 @@ int pick_bn(int N, long tiles_m) {
 
 int dispatch(int N, int bn, const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& b, TcParams& p,
              int tiles_m, int nbatch, cudaStream_t st, void* ws, size_t ws_bytes, size_t* query) {
-    // one persistent CTA per SM: TMA ring of 3-6 stages of one 64-wide K slab each (as many as fit next to the staging tile)
+    // one persistent CTA per SM: TMA ring of 4-6 stages of one 64-wide K slab each.  BN 160 takes 4, which fills the 227 KB
+    // next to the staging tile exactly: with 3 the deep-K convs waited on operand latency (DESIGN 3b, "Ring depth")
     p.tiles_n = (N + bn - 1) / bn;
     p.tiles_m = tiles_m;
     // split-K: non-batched, plain or SiLU epilogue, 16-byte aligned fp16/fp32 rows
@@ -588,7 +589,7 @@ int dispatch(int N, int bn, const CUtensorMap& a0, const CUtensorMap& a1, const 
         static_cast<long>(tiles_m) * p.tiles_n >= 4L * rf_num_sms() && !(env_bres && env_bres[0] == '0')) {
         return launch<160, 2, true>(a0, a1, b, p, grid, st);       // B-stationary (K <= 320, N = 160 k)
     }
-    if (bn == 160) rc = launch<160, 3>(a0, a1, b, p, grid, st);   // N = 320-type layers: two exact 160-column tiles
+    if (bn == 160) rc = launch<160, 4>(a0, a1, b, p, grid, st);   // N = 320-type layers: two exact 160-column tiles
     else if (bn == 128) rc = launch<128, 4>(a0, a1, b, p, grid, st);
     else rc = launch<64, 6>(a0, a1, b, p, grid, st);
     if (rc || p.splits == 1) return rc;
