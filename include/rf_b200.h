@@ -323,6 +323,12 @@ int rf_cfg_pndm_rows_step_f16(const void* eps_pair, int B, long m, const rf_pndm
 int rf_cfg_dpmpp_step_f16(const void* eps_pair, long n, float guidance, const void* sample, const void* m1,
                           float alpha_s0, float sigma_s0, float c_x, float c_0, float c_1, void* x0_out,
                           void* prev_sample, void* stream);
+/* rf_cfg_dpmpp_step_f16 for B rows of m elements that share one step's coefficients but each have their own guidance:
+ * d_guidance is a DEVICE array of B floats.  eps_pair: fp16 [2B][m] = [uncond | text]; sample, m1 (optional), x0_out,
+ * prev_sample: fp16 [B][m].  Row r gives the bits of rf_cfg_dpmpp_step_f16 run on that row with guidance d_guidance[r]. */
+int rf_cfg_dpmpp_rows_step_f16(const void* eps_pair, int B, long m, const float* d_guidance, const void* sample,
+                               const void* m1, float alpha_s0, float sigma_s0, float c_x, float c_0, float c_1,
+                               void* x0_out, void* prev_sample, void* stream);
 /* y = a*x + b*noise (scheduler.add_noise), optionally y = y*mask + z*(1-mask) (riffusion_pipeline.py:421-425) */
 int rf_axpby_f16(const void* x, const void* noise, float a, float b, const void* mask, const void* z, long n,
                  void* y, void* stream);

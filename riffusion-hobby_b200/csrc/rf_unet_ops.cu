@@ -728,13 +728,21 @@ __global__ void k_cfg_pndm_rows_step(const __half* __restrict__ eps_pair, int B,
 // x'  = c_x x + c_0 x0 + c_1 (x0 - m1)          first order (m1 == NULL) or the 2M midpoint update
 // x0 is rounded to fp16 once; x' is computed from that rounded x0, the value the next step reads back as m1.  Every
 // product and sum has an explicit rounding, so the result does not depend on how the compiler contracts.
-__global__ void k_cfg_dpmpp_step(const __half* __restrict__ eps_pair, size_t n, float guidance,
-                                 const __half* __restrict__ sample, const __half* __restrict__ m1, float alpha_s0,
-                                 float sigma_s0, float c_x, float c_0, float c_1, __half* __restrict__ x0_out,
-                                 __half* __restrict__ prev_sample) {
-    for (size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < n;
-         i += static_cast<size_t>(gridDim.x) * blockDim.x) {
-        const __half eu = eps_pair[i], et = eps_pair[n + i];
+// kRows: blockIdx.y = row r of gridDim.y rows of m elements each, guided with g_rows[r] (a text-to-audio batch whose
+// rows share every timestep but not the guidance); otherwise one row of m elements guided with `guidance`.  The
+// arithmetic is the same, so row r gives the bits of the scalar kernel run at g_rows[r].
+template <bool kRows>
+__global__ void k_cfg_dpmpp_step(const __half* __restrict__ eps_pair, size_t m, float guidance,
+                                 const float* __restrict__ g_rows, const __half* __restrict__ sample,
+                                 const __half* __restrict__ m1, float alpha_s0, float sigma_s0, float c_x, float c_0,
+                                 float c_1, __half* __restrict__ x0_out, __half* __restrict__ prev_sample) {
+    const size_t row0 = kRows ? static_cast<size_t>(blockIdx.y) * m : 0;
+    const size_t plane = kRows ? static_cast<size_t>(gridDim.y) * m : m;
+    if (kRows) guidance = g_rows[blockIdx.y];
+    for (size_t k = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x; k < m;
+         k += static_cast<size_t>(gridDim.x) * blockDim.x) {
+        const size_t i = row0 + k;
+        const __half eu = eps_pair[i], et = eps_pair[plane + i];
         const __half d = __hsub(et, eu);
         const __half gd = __float2half_rn(__half2float(d) * guidance);
         const float e = __half2float(__hadd(eu, gd));
@@ -1133,11 +1141,28 @@ extern "C" int rf_cfg_dpmpp_step_f16(const void* eps_pair, long n, float guidanc
                                      void* prev_sample, void* stream) {
     if (!eps_pair || !sample || !x0_out || !prev_sample || n <= 0 || !(alpha_s0 > 0.f))
         return rf_fail(RF_ERR_INVALID, "rf_cfg_dpmpp_step_f16: bad argument");
-    k_cfg_dpmpp_step<<<grid_for(static_cast<size_t>(n), 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
-        static_cast<const __half*>(eps_pair), static_cast<size_t>(n), guidance, static_cast<const __half*>(sample),
+    k_cfg_dpmpp_step<false><<<grid_for(static_cast<size_t>(n), 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+        static_cast<const __half*>(eps_pair), static_cast<size_t>(n), guidance, nullptr,
+        static_cast<const __half*>(sample), static_cast<const __half*>(m1), alpha_s0, sigma_s0, c_x, c_0, c_1,
+        static_cast<__half*>(x0_out), static_cast<__half*>(prev_sample));
+    RF_CUDA_LAUNCH_CHECK("k_cfg_dpmpp_step");
+    return RF_OK;
+}
+
+extern "C" int rf_cfg_dpmpp_rows_step_f16(const void* eps_pair, int B, long m, const float* d_guidance,
+                                          const void* sample, const void* m1, float alpha_s0, float sigma_s0, float c_x,
+                                          float c_0, float c_1, void* x0_out, void* prev_sample, void* stream) {
+    if (!eps_pair || !d_guidance || !sample || !x0_out || !prev_sample || B <= 0 || B > 65535 || m <= 0 ||
+        !(alpha_s0 > 0.f))
+        return rf_fail(RF_ERR_INVALID, "rf_cfg_dpmpp_rows_step_f16: bad argument");
+    const size_t per_row = static_cast<size_t>(m);
+    // the grid-stride budget of the whole batch, split evenly over the rows (as rf_cfg_pndm_rows_step_f16)
+    const unsigned bx = std::max(1u, grid_for(per_row * B, 256) / static_cast<unsigned>(B));
+    k_cfg_dpmpp_step<true><<<dim3(bx, static_cast<unsigned>(B)), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+        static_cast<const __half*>(eps_pair), per_row, 0.f, d_guidance, static_cast<const __half*>(sample),
         static_cast<const __half*>(m1), alpha_s0, sigma_s0, c_x, c_0, c_1, static_cast<__half*>(x0_out),
         static_cast<__half*>(prev_sample));
-    RF_CUDA_LAUNCH_CHECK("k_cfg_dpmpp_step");
+    RF_CUDA_LAUNCH_CHECK("k_cfg_dpmpp_rows_step");
     return RF_OK;
 }
 

@@ -124,6 +124,9 @@ SIGNATURES = {
                                             C.c_void_p, C.c_void_p, C.c_void_p]),
     "rf_cfg_dpmpp_step_f16": (C.c_int, [C.c_void_p, C.c_long, C.c_float, C.c_void_p, C.c_void_p, C.c_float, C.c_float,
                                         C.c_float, C.c_float, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "rf_cfg_dpmpp_rows_step_f16": (C.c_int, [C.c_void_p, C.c_int, C.c_long, C.c_void_p, C.c_void_p, C.c_void_p,
+                                             C.c_float, C.c_float, C.c_float, C.c_float, C.c_float, C.c_void_p,
+                                             C.c_void_p, C.c_void_p]),
     "rf_axpby_f16": (C.c_int, [C.c_void_p, C.c_void_p, C.c_float, C.c_float, C.c_void_p, C.c_void_p, C.c_long,
                                C.c_void_p, C.c_void_p]),
     "rf_magic_mix_f16": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_float, C.c_float, C.c_float, C.c_long,

@@ -21,6 +21,8 @@ the same names, flags and defaults (`COMMANDS`, what `build_parser()` builds by 
         [--image-dir steps] [--seed-a 42] [--seed-b 42] [--denoising-a 0.75] [--denoising-b 0.75] [--guidance 7.0]
         [--num-interpolation-steps 12] [--num-inference-steps 50] [--alpha-power 1.0] [--max-batch 32]
         [--checkpoint DIR] [--device cuda]
+    python -m riffusion.cli text-to-audio-batch --json inputs.json --output-dir out [--num-seeds 1] [--max-batch 32]
+        [--audio-extension wav] [--checkpoint DIR] [--device cuda]
 
 `text-to-audio` loads a local diffusers-layout checkpoint directory; with `--num-clips N` > 1 clip i (seed + i) is
 written to out_<seed + i>.wav / .png.  The image carries the spectrogram parameters in its EXIF block, so
@@ -296,11 +298,43 @@ def interpolation(*, prompt_a: str, prompt_b: str, seed_image: str, output: str,
         print(f"Wrote {len(out['alphas'])} images to {image_dir}")
 
 
+def text_to_audio_batch(*, json: str, output_dir: str, num_seeds: int = 1, max_batch: int = 32,
+                        audio_extension: str = "wav", checkpoint: str = "riffusion/riffusion-model-v1",
+                        device: str = "cuda"):
+    """Generate audio for every (entry, seed, param set) of a JSON file of param sets and prompts (the app's Text to
+    Audio Batch format), writing image_*.jpg / audio_* per clip and index.json to --output-dir."""
+    import json as json_module
+
+    from riffusion.riffusion_pipeline import DEFAULT_PARAMS, RiffusionPipeline
+    from riffusion.text_to_audio_batch import build_index, output_names, parse_batch, plan_batch
+
+    data = json_module.loads(Path(json).read_text())
+    param_sets, entries = parse_batch(data)
+    clips, _ = plan_batch(param_sets, entries, num_seeds, max_batch)      # refuses bad counts before loading weights
+    for ps in param_sets:
+        if ps.checkpoint != checkpoint:
+            print(f"{ps.name}: names checkpoint {ps.checkpoint!r}; every clip runs on {checkpoint!r}")
+    pipe = RiffusionPipeline.load_checkpoint(checkpoint=checkpoint, device=device)
+    out = pipe.text_to_audio_batch(data, num_seeds=num_seeds, max_batch=max_batch)
+    target = Path(output_dir)
+    target.mkdir(parents=True, exist_ok=True)
+    paths = []
+    for clip, res in zip(clips, out["clips"]):
+        image_name, audio_name = output_names(clip.param_index, entries[clip.entry_index], clip.seed, audio_extension)
+        _store_spectrogram(res["image"].cpu().numpy(), DEFAULT_PARAMS, target / image_name, "JPEG")
+        res["segment"].export(str(target / audio_name), format=audio_extension)
+        paths.append((str(target / image_name), str(target / audio_name)))
+    (target / "index.json").write_text(json_module.dumps(build_index(data, param_sets, clips, paths), indent=4))
+    print(f"Wrote {len(clips)} clips in {len(out['loops'])} loops and index.json to {output_dir}")
+
+
 COMMANDS = [audio_to_image, image_to_audio, sample_clips, print_exif, audio_to_images_batch, sample_clips_batch]
 # commands of this package that the reference's CLI does not have; `main` offers them next to COMMANDS
 EXTRA_COMMANDS = [text_to_audio]
 # the track-level commands, offered by `main` after EXTRA_COMMANDS
 TRACK_COMMANDS = [audio_to_audio, interpolation]
+# the file-driven batch commands, offered by `main` after TRACK_COMMANDS
+BATCH_COMMANDS = [text_to_audio_batch]
 
 
 # ------------------------------------------------------------------------------------------------ argparse front end
@@ -334,7 +368,7 @@ def build_parser(commands: T.Sequence[T.Callable] = tuple(COMMANDS)) -> argparse
 
 
 def main(argv: T.Optional[T.Sequence[str]] = None) -> None:
-    args = vars(build_parser(COMMANDS + EXTRA_COMMANDS + TRACK_COMMANDS).parse_args(argv))
+    args = vars(build_parser(COMMANDS + EXTRA_COMMANDS + TRACK_COMMANDS + BATCH_COMMANDS).parse_args(argv))
     fn = args.pop("_fn")
     args.pop("command")
     fn(**args)

@@ -659,6 +659,66 @@ class RiffusionPipeline:
         return dict(images=u8, waveform=wave, latents=out["latents"], latents_unscaled=out["latents_unscaled"],
                     n_unet_evals=out["n_unet_evals"])
 
+    @torch.no_grad()
+    def text_to_audio_batch(self, batch: dict, *, num_seeds: int = 1, max_batch: int = 32, converter=None,
+                            apply_filters: bool = True) -> T.Dict[str, T.Any]:
+        """The app's Text to Audio Batch task (streamlit/tasks/text_to_audio_batch.py) on a loaded batch JSON object
+        (format: `riffusion.text_to_audio_batch`).  For every (entry, seed, param set), in that order, the clip is
+        `txt2img` of the entry's prompt / negative prompt at that seed with the set's steps, guidance, width and
+        scheduler, at height 512, turned into mono 0-10 kHz audio.  The param sets' `checkpoint` is not loaded: every
+        clip runs on this pipeline.
+
+        Clips are grouped into loops by `text_to_audio_batch.plan_batch` (same scheduler, steps, width and side of
+        guidance 1; at most `max_batch` rows), and each loop is one CFG loop whose rows keep their own guidance
+        (`DPMSolverRowsB200` / `PNDMRowsB200`).  Row r starts from `torch.randn((1, 4, 64, W/8))` drawn from a CUDA
+        generator seeded with its seed, with context [embed_text(negative or "") | embed_text(prompt)], exactly
+        txt2img's draws.  After each loop, on the device: VAE decode -> uint8 image -> mel -> waveform; on the host:
+        peak-normalised int16 and, with `apply_filters`, `apply_filters(compression=False)`.
+
+        Raises ValueError before any device work for a malformed batch, num_seeds or max_batch below 1.  Returns
+        dict(clips, loops): per clip (in the app's order) param_index, param_name, entry_index, seed, prompt,
+        negative_prompt, latents_unscaled ((4, 64, W/8) fp16, the loop's output), image ((512, W, 3) uint8), waveform
+        ((1, L) fp32 before normalisation), all device tensors, and segment (AudioSegment); per loop rows (clip
+        indices), scheduler, num_inference_steps, width, n_unet_evals."""
+        from riffusion.scheduler_b200 import DPMSolverRowsB200, PNDMRowsB200
+        from riffusion.text_to_audio_batch import parse_batch, plan_batch
+        from riffusion.util import audio_util
+
+        param_sets, entries = parse_batch(batch)
+        clips, loops = plan_batch(param_sets, entries, num_seeds, max_batch)
+        params = DEFAULT_PARAMS
+        converter = self._converter(params, converter)
+        out_clips: T.List[T.Optional[dict]] = [None] * len(clips)
+        out_loops = []
+        for loop in loops:
+            rows = [clips[k] for k in loop.rows]
+            guidances = [param_sets[c.param_index].guidance for c in rows]
+            texts = torch.cat([self.embed_text(entries[c.entry_index].prompt) for c in rows])
+            unconds = torch.cat([self.embed_text(entries[c.entry_index].negative_prompt or "") for c in rows])
+            context = self._context(None, None, len(rows), loop.cfg, texts, unconds)
+            shape = (1, 4, params.num_frequencies // 8, loop.width // 8)
+            latents = torch.cat([torch.randn(shape, generator=torch.Generator(device=self.device).manual_seed(c.seed),
+                                             device=self.device, dtype=torch.float16) for c in rows]).contiguous()
+            if loop.scheduler == "PNDMScheduler":
+                sched = PNDMRowsB200(loop.num_inference_steps, [0] * len(rows), guidances, device=self._device)
+            else:
+                sched = DPMSolverRowsB200(loop.num_inference_steps, guidances, device=self._device)
+            latents, n_evals = self._denoise(sched, sched.timesteps, latents, context, guidances[0])
+            u8 = self._decode_u8((1.0 / VAE_SCALE) * latents)
+            wave = self._u8_to_waveform(u8, converter, params.stereo, None)
+            for j, (k, c) in enumerate(zip(loop.rows, rows)):
+                seg = audio_util.audio_from_waveform(samples=wave[j].cpu().numpy(), sample_rate=params.sample_rate,
+                                                     normalize=True)
+                entry = entries[c.entry_index]
+                out_clips[k] = dict(param_index=c.param_index, param_name=param_sets[c.param_index].name,
+                                    entry_index=c.entry_index, seed=c.seed, prompt=entry.prompt,
+                                    negative_prompt=entry.negative_prompt, latents_unscaled=latents[j], image=u8[j],
+                                    waveform=wave[j],
+                                    segment=audio_util.apply_filters(seg, compression=False) if apply_filters else seg)
+            out_loops.append(dict(rows=list(loop.rows), scheduler=loop.scheduler,
+                                  num_inference_steps=loop.num_inference_steps, width=loop.width, n_unet_evals=n_evals))
+        return dict(clips=out_clips, loops=out_loops)
+
     def _converter(self, params, converter):
         """`converter`, which must have been built for `params`, or a new SpectrogramConverter for them on this
         pipeline's device."""

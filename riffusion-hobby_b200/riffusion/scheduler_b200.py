@@ -130,6 +130,15 @@ ROW_BASE_SAVED, ROW_SAVE = 1, 2           # RF_PNDM_ROW_BASE_SAVED, RF_PNDM_ROW_
 _SAVED = "saved"                          # the token `advance` keeps as a row's first sample
 
 
+def rows_guidance(guidances: T.Sequence[float]) -> T.List[float]:
+    """The guidance a rows step applies to each row: the row's own when every row is above 1, else 0 for every row (the
+    loop then passes [eps | eps]).  Raises ValueError when the rows lie on both sides of 1."""
+    cfg = {float(g) > 1.0 for g in guidances}
+    if len(cfg) != 1:
+        raise ValueError("the rows' guidance lies on both sides of 1: only some rows would use guidance")
+    return [float(g) for g in guidances] if cfg == {True} else [0.0] * len(guidances)
+
+
 def cfg_pndm_rows_step(eps_pair: torch.Tensor, rows: torch.Tensor, ring: torch.Tensor, saved: torch.Tensor,
                        sample: torch.Tensor) -> torch.Tensor:
     """One PLMS step of B rows with per-row state (`rf_cfg_pndm_rows_step_f16`).  eps_pair: (2B, ...) fp16 [uncond |
@@ -167,10 +176,7 @@ class PNDMRowsB200:
                  device="cuda"):
         if len(t_starts) != len(guidances) or not len(t_starts):
             raise ValueError(f"need one t_start and one guidance per row, got {len(t_starts)} and {len(guidances)}")
-        cfg = {float(g) > 1.0 for g in guidances}
-        if len(cfg) != 1:
-            raise ValueError("the rows' guidance lies on both sides of 1: only some rows would use guidance")
-        use_cfg = cfg.pop()
+        guidances = rows_guidance(guidances)
         ref = PNDMSchedulerB200()
         ref.set_timesteps(num_inference_steps)
         self.all_timesteps = ref.timesteps
@@ -190,7 +196,7 @@ class PNDMRowsB200:
                 coef, hist, override, push, ca, cb = s.plan(int(self.all_timesteps[i]))
                 rec = table[i - self.t0, r]
                 rec["active"] = 1
-                rec["guidance"] = float(g) if use_cfg else 0.0
+                rec["guidance"] = g
                 rec["c0"], rec["c1"], rec["c2"], rec["c3"] = coef
                 rec["ca"], rec["cb"] = ca, cb
                 for name, slot in zip(("h1", "h2", "h3"), hist):
@@ -281,10 +287,55 @@ class DPMSolverMultistepSchedulerB200(_ScaledLinearScheduler):
         """Guidance combine + DPMSolverMultistepScheduler.step in one kernel.  eps_pair = UNet output for [uncond | text]."""
         order, coefs = self.plan(timestep)
         m1 = self.model_outputs[-1] if order == 2 else None
-        x0, prev = ops.cfg_dpmpp_step(eps_pair.contiguous(), guidance, sample.contiguous(), m1, coefs)
+        x0, prev = self._fused_step(eps_pair.contiguous(), guidance, sample.contiguous(), m1, coefs)
         self.model_outputs = self.model_outputs[1:] + [x0]
         self.lower_order_nums = min(self.lower_order_nums + 1, self.config["solver_order"])
         return prev
+
+    def _fused_step(self, eps_pair, guidance, sample, m1, coefs):
+        return ops.cfg_dpmpp_step(eps_pair, guidance, sample, m1, coefs)
+
+
+def cfg_dpmpp_rows_step(eps_pair: torch.Tensor, guidance_rows: torch.Tensor, sample: torch.Tensor,
+                        m1: T.Optional[torch.Tensor], coefs) -> T.Tuple[torch.Tensor, torch.Tensor]:
+    """Guidance combine + one DPM-Solver++ update of B rows, row r guided with guidance_rows[r]
+    (`rf_cfg_dpmpp_rows_step_f16`).  eps_pair: (2B, ...) fp16 [uncond | text]; guidance_rows: (B,) fp32; sample: (B, ...)
+    fp16; m1: the previous step's x0 shaped like sample, or None (first order); coefs = (alpha_s0, sigma_s0, c_x, c_0,
+    c_1), shared by every row.  Returns (x0, prev_sample)."""
+    operand(sample, "sample", torch.float16)
+    dev = sample.device
+    if sample.dim() < 1 or sample.numel() == 0:
+        raise ValueError(f"sample must hold at least one element per row, got shape {tuple(sample.shape)}")
+    B = sample.shape[0]
+    operand(eps_pair, "eps_pair", torch.float16, shape=(2 * B, *sample.shape[1:]), device=dev)
+    operand(guidance_rows, "guidance_rows", torch.float32, shape=(B,), device=dev)
+    if m1 is not None:
+        operand(m1, "m1", torch.float16, shape=sample.shape, device=dev)
+    alpha_s0, sigma_s0, c_x, c_0, c_1 = (float(v) for v in coefs)
+    x0 = torch.empty_like(sample)
+    prev = torch.empty_like(sample)
+    _native.call("rf_cfg_dpmpp_rows_step_f16", dev, eps_pair.data_ptr(), B, sample.numel() // B,
+                 guidance_rows.data_ptr(), sample.data_ptr(), _native.ptr(m1), alpha_s0, sigma_s0, c_x, c_0, c_1,
+                 x0.data_ptr(), prev.data_ptr())
+    return x0, prev
+
+
+class DPMSolverRowsB200(DPMSolverMultistepSchedulerB200):
+    """`DPMSolverMultistepSchedulerB200` over `num_inference_steps` for B rows that each keep their own guidance:
+    `RiffusionPipeline._denoise` drives it in place of a scheduler, and every row runs the same timesteps from the
+    first.  The plan and the x0 history are the parent's; only the fused step differs, one `rf_cfg_dpmpp_rows_step_f16`
+    launch per step with the rows' guidance held on the device (`rows_guidance`: each row's above 1, else 0 for every
+    row).  The guidance scalar the loop passes is not used."""
+
+    def __init__(self, num_inference_steps: int, guidances: T.Sequence[float], device="cuda"):
+        if not len(guidances):
+            raise ValueError("need one guidance per row, got none")
+        super().__init__()
+        self.set_timesteps(num_inference_steps)
+        self.guidance = torch.tensor(rows_guidance(guidances), dtype=torch.float32, device=device)
+
+    def _fused_step(self, eps_pair, guidance, sample, m1, coefs):
+        return cfg_dpmpp_rows_step(eps_pair, self.guidance, sample, m1, coefs)
 
 
 SCHEDULERS = {"DPMSolverMultistepScheduler": DPMSolverMultistepSchedulerB200, "PNDMScheduler": PNDMSchedulerB200}
