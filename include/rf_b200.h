@@ -329,6 +329,15 @@ int rf_cfg_dpmpp_step_f16(const void* eps_pair, long n, float guidance, const vo
 int rf_cfg_dpmpp_rows_step_f16(const void* eps_pair, int B, long m, const float* d_guidance, const void* sample,
                                const void* m1, float alpha_s0, float sigma_s0, float c_x, float c_0, float c_1,
                                void* x0_out, void* prev_sample, void* stream);
+/* classifier-free guidance + one Euler-ancestral step on B rows of m elements:
+ *   eps = eps_u + g (eps_t - eps_u) (fp16, as rf_cfg_pndm_step_f16); prev = x + dt eps + sigma_up z.
+ *   g is d_guidance_rows[r] for row r when that DEVICE array of B floats is given, else `guidance`.  The host passes
+ *   dt = sigma_down - sigma and sigma_up of EulerAncestralDiscreteScheduler.step; noise z (optional, NULL = no z term)
+ *   is fp16 [B][m].  eps_pair: fp16 [2B][m] = [uncond | text]; sample, prev_sample: fp16 [B][m] in sigma space.  fp32
+ *   math with explicit roundings, one fp16 rounding of prev; row r gives the bits of a launch with guidance g[r]. */
+int rf_cfg_euler_a_step_f16(const void* eps_pair, int B, long m, float guidance, const float* d_guidance_rows,
+                            const void* sample, const void* noise, float dt, float sigma_up, void* prev_sample,
+                            void* stream);
 /* y = a*x + b*noise (scheduler.add_noise), optionally y = y*mask + z*(1-mask) (riffusion_pipeline.py:421-425) */
 int rf_axpby_f16(const void* x, const void* noise, float a, float b, const void* mask, const void* z, long n,
                  void* y, void* stream);

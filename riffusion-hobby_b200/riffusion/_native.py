@@ -127,6 +127,8 @@ SIGNATURES = {
     "rf_cfg_dpmpp_rows_step_f16": (C.c_int, [C.c_void_p, C.c_int, C.c_long, C.c_void_p, C.c_void_p, C.c_void_p,
                                              C.c_float, C.c_float, C.c_float, C.c_float, C.c_float, C.c_void_p,
                                              C.c_void_p, C.c_void_p]),
+    "rf_cfg_euler_a_step_f16": (C.c_int, [C.c_void_p, C.c_int, C.c_long, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p,
+                                          C.c_float, C.c_float, C.c_void_p, C.c_void_p]),
     "rf_axpby_f16": (C.c_int, [C.c_void_p, C.c_void_p, C.c_float, C.c_float, C.c_void_p, C.c_void_p, C.c_long,
                                C.c_void_p, C.c_void_p]),
     "rf_magic_mix_f16": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_float, C.c_float, C.c_float, C.c_long,

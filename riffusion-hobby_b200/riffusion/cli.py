@@ -24,7 +24,8 @@ the same names, flags and defaults (`COMMANDS`, what `build_parser()` builds by 
     python -m riffusion.cli text-to-audio-batch --json inputs.json --output-dir out [--num-seeds 1] [--max-batch 32]
         [--audio-extension wav] [--checkpoint DIR] [--device cuda]
 
-`text-to-audio` loads a local diffusers-layout checkpoint directory; with `--num-clips N` > 1 clip i (seed + i) is
+`--scheduler` takes DPMSolverMultistepScheduler, PNDMScheduler, DDIMScheduler or EulerAncestralDiscreteScheduler
+(audio-to-audio's --magic-mix refuses the last).  `text-to-audio` loads a local diffusers-layout checkpoint directory; with `--num-clips N` > 1 clip i (seed + i) is
 written to out_<seed + i>.wav / .png.  The image carries the spectrogram parameters in its EXIF block, so
 `image-to-audio` turns it back into the same audio.
 

@@ -24,7 +24,8 @@ from PIL import Image
 
 from riffusion import tc_ops as ops
 from riffusion.datatypes import InferenceInput
-from riffusion.scheduler_b200 import PNDMSchedulerB200, make_scheduler
+from riffusion.scheduler_b200 import (DDIMSchedulerB200, EulerAncestralSchedulerB200, PNDMSchedulerB200,
+                                      make_scheduler)
 from riffusion.spectrogram_params import SpectrogramParams
 from riffusion.unet_b200 import UNetB200
 from riffusion.util import torch_util
@@ -337,9 +338,14 @@ class RiffusionPipeline:
                             noise: T.Optional[torch.Tensor] = None, **kwargs) -> T.Dict[str, T.Any]:
         """riffusion_pipeline.py:289-436.  Extra keyword-only inputs (`uncond_embeddings`, `noise_a`, `noise_b`)
         let callers inject what the reference computes internally (CLIP("") and the generator draws) — used by
-        the parity tests and by runs without a text encoder."""
+        the parity tests and by runs without a text encoder.  The pipeline's scheduler may be PNDM (eta is ignored, as
+        the reference's PNDM ignores it) or DDIM (eta must be 0; ValueError otherwise)."""
         batch_size = text_embeddings.shape[0]
         sched = self.scheduler
+        if isinstance(sched, EulerAncestralSchedulerB200):
+            raise ValueError("interpolate_img2img runs PNDM or DDIM; Euler ancestral needs per-step noise (use img2img)")
+        if eta and isinstance(sched, DDIMSchedulerB200):
+            raise ValueError(f"DDIM runs with eta = 0 only, got eta {eta}")
         sched.set_timesteps(num_inference_steps)
         dev = self._device
         text_embeddings = text_embeddings.to(device=dev, dtype=torch.float16)
@@ -413,15 +419,19 @@ class RiffusionPipeline:
                 num_inference_steps: int = 30, guidance_scale: float = 7.0, width: int = 512, height: int = 512,
                 scheduler: str = "DPMSolverMultistepScheduler", output_type: T.Optional[str] = "pil",
                 text_embeddings: T.Optional[torch.Tensor] = None, uncond_embeddings: T.Optional[torch.Tensor] = None,
-                latents: T.Optional[torch.Tensor] = None) -> T.Dict[str, T.Any]:
+                latents: T.Optional[torch.Tensor] = None,
+                step_noise: T.Optional[torch.Tensor] = None) -> T.Dict[str, T.Any]:
         """Text to spectrogram image: Stable Diffusion txt2img, the reference app's text-to-audio generation.
 
         Clip i starts from `torch.randn((1, 4, height/8, width/8))` drawn from a CUDA generator seeded with `seed + i`
-        (one pipeline call per seed in the app); all clips run as one CFG batch.  The prompt and the negative prompt
-        (default "") are encoded without prompt weighting.  `scheduler` is "DPMSolverMultistepScheduler" or
-        "PNDMScheduler"; a fresh instance is used per call.  `width` and `height` must be multiples of 64 (diffusers
-        accepts multiples of 8).  `text_embeddings` / `uncond_embeddings` / `latents` replace the text encoder and the
-        generator draws.  Returns dict(images, latents (1/0.18215-scaled), latents_unscaled, n_unet_evals)."""
+        (one pipeline call per seed in the app), times the scheduler's `init_noise_sigma`; all clips run as one CFG
+        batch.  The prompt and the negative prompt (default "") are encoded without prompt weighting.  `scheduler` is
+        "DPMSolverMultistepScheduler", "PNDMScheduler", "DDIMScheduler" or "EulerAncestralDiscreteScheduler"; a fresh
+        instance is used per call.  Euler ancestral also draws one fp16 tensor per step from each clip's generator,
+        after its latents (`_step_noise`).  `width` and `height` must be multiples of 64 (diffusers accepts multiples of
+        8).  `text_embeddings` / `uncond_embeddings` / `latents` / `step_noise` (steps, clips, 4, h, w) replace the text
+        encoder and the generator draws.  Returns dict(images, latents (1/0.18215-scaled), latents_unscaled,
+        n_unet_evals)."""
         if width <= 0 or height <= 0 or width % 64 or height % 64:
             raise ValueError(f"width and height must be positive multiples of 64, got {width}x{height}")
         if num_clips < 1:
@@ -432,12 +442,13 @@ class RiffusionPipeline:
         context = self._context(prompt, negative_prompt, num_clips, guidance_scale > 1.0, text_embeddings,
                                 uncond_embeddings)
         shape = (1, 4, height // 8, width // 8)
+        gens = [torch.Generator(device=self.device).manual_seed(seed + i) for i in range(num_clips)]
         if latents is None:
-            latents = torch.cat([torch.randn(shape, generator=torch.Generator(device=self.device).manual_seed(seed + i),
-                                             device=self.device, dtype=torch.float16) for i in range(num_clips)])
+            latents = torch.cat([torch.randn(shape, generator=g, device=self.device, dtype=torch.float16) for g in gens])
         latents = latents.to(device=dev, dtype=torch.float16).contiguous()
         if tuple(latents.shape) != (num_clips,) + shape[1:]:
             raise ValueError(f"latents must be {(num_clips,) + shape[1:]}, got {tuple(latents.shape)}")
+        self._step_noise(sched, len(sched.timesteps), latents, step_noise, gens)
         if sched.init_noise_sigma != 1.0:
             latents = (latents * sched.init_noise_sigma).contiguous()
         latents, n_evals = self._denoise(sched, sched.timesteps, latents, context, guidance_scale)
@@ -462,6 +473,29 @@ class RiffusionPipeline:
         uncond = self.embed_text(negative_prompt or "") if uncond_embeddings is None else uncond_embeddings
         return torch.cat([rows(uncond, "uncond_embeddings"), text]).contiguous()
 
+    def _step_noise(self, sched, n_steps: int, latents: torch.Tensor, step_noise: T.Optional[torch.Tensor],
+                    generators: T.Sequence[torch.Generator]) -> None:
+        """Hand an Euler-ancestral scheduler the z of each of the loop's `n_steps` steps, (n_steps, B, ...) fp16:
+        `step_noise` when given, else n_steps draws of torch.randn((1, ...), fp16) per row from that row's generator,
+        continuing its stream, as diffusers' step draws them from the pipeline's generator.  One generator for B rows
+        means the rows' streams are identical (img2img seeds every image alike) and its draws serve every row.  Other
+        schedulers draw nothing and take no step_noise (ValueError)."""
+        if not isinstance(sched, EulerAncestralSchedulerB200):
+            if step_noise is not None:
+                raise ValueError("step_noise is only used by EulerAncestralDiscreteScheduler")
+            return
+        want = (n_steps,) + tuple(latents.shape)
+        if step_noise is None:
+            row = (1,) + tuple(latents.shape[1:])
+            draws = [torch.cat([torch.randn(row, generator=g, device=self.device, dtype=torch.float16)
+                                for _ in range(n_steps)]) if n_steps else latents.new_empty((0,) + row[1:])
+                     for g in generators]
+            step_noise = torch.stack(draws, dim=1) if len(draws) > 1 else draws[0][:, None].expand(want)
+        step_noise = step_noise.to(device=latents.device, dtype=torch.float16).contiguous()
+        if tuple(step_noise.shape) != want:
+            raise ValueError(f"step_noise must be {want}, got {tuple(step_noise.shape)}")
+        sched.set_step_noise(step_noise)
+
     def _denoise(self, sched, timesteps, latents: torch.Tensor, context: torch.Tensor, guidance_scale: float,
                  mask: T.Optional[torch.Tensor] = None, init: T.Optional[torch.Tensor] = None,
                  noise: T.Optional[torch.Tensor] = None,
@@ -471,7 +505,10 @@ class RiffusionPipeline:
         interpolate_img2img (:420-425): `init` noised with `noise` at that step's timestep where the mask is 1, the
         stepped latents where it is 0.  With `layout` = (mix_factor, enc, noise32, stop), steps 1 .. stop - 1 of the
         loop are Magic Mix's layout phase: the UNet evaluates mix_factor * latents + (1 - mix_factor) * add_noise(enc,
-        noise32, t) (`tc_ops.magic_mix`) and the scheduler still steps the latents.  Returns (latents, evaluations)."""
+        noise32, t) (`tc_ops.magic_mix`) and the scheduler still steps the latents.  The UNet input passes through
+        `sched.scale_model_input` (the identity, without a launch, for every scheduler but Euler ancestral).  The UNet,
+        the graph and the scheduler receive the scheduler's own timestep values: ints, or floats for Euler ancestral.
+        Returns (latents, evaluations)."""
         do_cfg = guidance_scale > 1.0
         ctx_cache: T.Dict[str, T.Any] = {}
         graphed = self._graphed_unet(latents.shape, context) if do_cfg else None
@@ -479,22 +516,23 @@ class RiffusionPipeline:
             mask = mask.to(device=latents.device, dtype=latents.dtype).expand_as(latents).contiguous()
         n_evals = 0
         for j, t in enumerate(timesteps):
-            t_int = int(t)
+            t_val = t.item() if torch.is_tensor(t) else t
             unet_in = latents
             if layout is not None and 0 < j < layout[3]:
-                a = float(sched.alphas_cumprod[t_int])
+                a = float(sched.alphas_cumprod[t_val])
                 unet_in = ops.magic_mix(latents, layout[1], layout[2], a ** 0.5, (1.0 - a) ** 0.5, layout[0])
+            unet_in = sched.scale_model_input(unet_in, t_val)
             if graphed is not None:
-                eps_pair = graphed(unet_in, t_int)
+                eps_pair = graphed(unet_in, t_val)
             else:
                 model_in = torch.cat([unet_in] * 2) if do_cfg else unet_in
-                eps_pair = self.unet(model_in, t_int, encoder_hidden_states=context, ctx_cache=ctx_cache).sample
+                eps_pair = self.unet(model_in, t_val, encoder_hidden_states=context, ctx_cache=ctx_cache).sample
             n_evals += 1
             if not do_cfg:
                 eps_pair = torch.cat([eps_pair, eps_pair])
-            latents = sched.step_cfg(eps_pair, guidance_scale if do_cfg else 0.0, t_int, latents)
+            latents = sched.step_cfg(eps_pair, guidance_scale if do_cfg else 0.0, t_val, latents)
             if mask is not None:
-                latents = sched.add_noise(init, noise, t_int, mask=mask, blend_with=latents)
+                latents = sched.add_noise(init, noise, t_val, mask=mask, blend_with=latents)
         return latents, n_evals
 
     def _finish(self, latents: torch.Tensor, n_evals: int, output_type: T.Optional[str]) -> T.Dict[str, T.Any]:
@@ -523,17 +561,22 @@ class RiffusionPipeline:
                 seed: int = 42, scheduler: str = "DPMSolverMultistepScheduler", output_type: T.Optional[str] = "pil",
                 text_embeddings: T.Optional[torch.Tensor] = None, uncond_embeddings: T.Optional[torch.Tensor] = None,
                 noise: T.Optional[torch.Tensor] = None,
-                moments: T.Optional[T.Tuple[torch.Tensor, torch.Tensor]] = None) -> T.Dict[str, T.Any]:
+                moments: T.Optional[T.Tuple[torch.Tensor, torch.Tensor]] = None,
+                step_noise: T.Optional[torch.Tensor] = None) -> T.Dict[str, T.Any]:
         """Image to image: diffusers' StableDiffusionImg2ImgPipeline as the reference app calls it
         (streamlit/util.py:354-396), for a batch of images in one CFG loop.
 
         `images`: PIL images (preprocessed like `preprocess_image`) or a (B, 3, H, W) fp16 device tensor in [-1, 1]; H and
         W must be multiples of 64.  Image i is denoised with its own generator seeded with `seed` (the app uses one seed
         for every clip), which draws the VAE posterior noise (fp32) first and then the img2img noise (fp16).  The start
-        point follows `img2img_start` (unpinned for DPM-Solver++): noise is added at timesteps[t_start], then
-        timesteps[t_start:] are run.  `scheduler`: "DPMSolverMultistepScheduler" or "PNDMScheduler", a fresh instance per
-        call.  `text_embeddings` / `uncond_embeddings` / `noise` (B, 4, H/8, W/8) replace the text encoder and the
-        img2img noise draw; `moments` = (mean, logvar) replaces the VAE encoding of `images` (pass None for them).
+        point follows `img2img_start` (unpinned for DPM-Solver++, DDIM and Euler ancestral): noise is added at
+        timesteps[t_start], then timesteps[t_start:] are run.  `scheduler`: "DPMSolverMultistepScheduler",
+        "PNDMScheduler", "DDIMScheduler" or "EulerAncestralDiscreteScheduler", a fresh instance per call; Euler ancestral
+        then draws one fp16 tensor per step run from the same generator, after the img2img noise, and since every image's
+        generator has drawn the same shapes from the same seed, one stream serves all images.  `text_embeddings` /
+        `uncond_embeddings` / `noise` (B, 4, H/8, W/8) / `step_noise` (steps run, B, 4, H/8, W/8) replace the text
+        encoder and the generator draws; `moments` = (mean, logvar) replaces the VAE encoding of `images` (pass None for
+        them).
         Returns dict(images, latents (1/0.18215-scaled), latents_unscaled, n_unet_evals, t_start)."""
         sched = make_scheduler(scheduler)
         sched.set_timesteps(num_inference_steps)
@@ -546,15 +589,17 @@ class RiffusionPipeline:
             g = torch.Generator(device=self.device).manual_seed(seed)
             lats.append(_sample_latents(mean[i:i + 1], logvar[i:i + 1], g))
             draws.append(torch.randn(lats[-1].shape, generator=g, device=self.device, dtype=torch.float16))
+        stream = g                          # the state every image's generator is in now
         init_latents = torch.cat(lats).to(device=dev, dtype=torch.float16).contiguous()
         noise = torch.cat(draws) if noise is None else noise.to(device=dev, dtype=torch.float16)
         if noise.shape != init_latents.shape:
             raise ValueError(f"noise must be {tuple(init_latents.shape)}, got {tuple(noise.shape)}")
         t_start = self.img2img_start(sched, num_inference_steps, strength)
         timesteps = sched.timesteps[t_start:]
+        self._step_noise(sched, len(timesteps), init_latents, step_noise, [stream])
         latents = init_latents
         if len(timesteps):
-            latents = sched.add_noise(init_latents, noise, int(timesteps[0]))
+            latents = sched.add_noise(init_latents, noise, timesteps[0].item())
         latents, n_evals = self._denoise(sched, timesteps, latents, context, guidance_scale)
         out = self._finish(latents, n_evals, output_type)
         out["t_start"] = t_start
@@ -583,6 +628,12 @@ class RiffusionPipeline:
             raise ValueError(f"kmax must be at most 1, got {kmax}")
         return n - int(kmax * n), n - int(kmin * n)
 
+    @staticmethod
+    def _check_magic_mix_scheduler(scheduler: str) -> None:
+        if scheduler == "EulerAncestralDiscreteScheduler":
+            raise ValueError("Magic Mix does not run EulerAncestralDiscreteScheduler: its layout blend noises in "
+                             "alpha-bar space, which a sigma-space scheduler does not use")
+
     @torch.no_grad()
     def magic_mix(self, prompt: str, images: T.Union[None, torch.Tensor, T.Sequence[Image.Image]], *, kmin: float = 0.3,
                   kmax: float = 0.5, mix_factor: float = 0.5, num_inference_steps: int = 25, guidance_scale: float = 7.0,
@@ -608,7 +659,10 @@ class RiffusionPipeline:
         unconditional context is embed_text(""): Magic Mix has no negative prompt.  `images`, `moments`,
         `text_embeddings`, `uncond_embeddings`, `scheduler` and `output_type` work as in `img2img`; an injected `noise`
         is (1 or B, 4, h, w).  Returns dict(images, latents (1/0.18215-scaled), latents_unscaled, n_unet_evals, t_max,
-        t_min); n_unet_evals = len(T) - t_max."""
+        t_min); n_unet_evals = len(T) - t_max.  DDIM runs like PNDM; Euler ancestral is refused (ValueError) before any
+        device work: the layout blend noises in ᾱ space, and how the community pipeline treats a sigma-space scheduler is
+        not known."""
+        self._check_magic_mix_scheduler(scheduler)
         t_max, t_min = self.magic_mix_range(num_inference_steps, kmin, kmax)
         sched = make_scheduler(scheduler)
         sched.set_timesteps(num_inference_steps)
@@ -640,10 +694,12 @@ class RiffusionPipeline:
                       height: T.Optional[int] = None, scheduler: str = "DPMSolverMultistepScheduler",
                       text_embeddings: T.Optional[torch.Tensor] = None, uncond_embeddings: T.Optional[torch.Tensor] = None,
                       latents: T.Optional[torch.Tensor] = None, converter=None,
-                      init_angles: T.Optional[torch.Tensor] = None) -> T.Dict[str, torch.Tensor]:
+                      init_angles: T.Optional[torch.Tensor] = None,
+                      step_noise: T.Optional[torch.Tensor] = None) -> T.Dict[str, torch.Tensor]:
         """Text to audio on the device: `txt2img` with height = params.num_frequencies, then VAE decode -> uint8 image ->
         mel amplitudes (`audio_from_spectrogram_image` semantics: R plane for mono, G and B for stereo, max_value 30e6)
-        -> inverse mel + Griffin-Lim.  `params` defaults to mono 0-10 kHz.  Returns device tensors: images (B, H, W, 3)
+        -> inverse mel + Griffin-Lim.  `params` defaults to mono 0-10 kHz; `scheduler`, `latents` and `step_noise` are
+        txt2img's.  Returns device tensors: images (B, H, W, 3)
         uint8, waveform (B, channels, hop * (W - 1)) fp32 before peak normalisation, latents, latents_unscaled,
         n_unet_evals."""
         params = DEFAULT_PARAMS if params is None else params
@@ -653,7 +709,8 @@ class RiffusionPipeline:
         out = self.txt2img(prompt, negative_prompt=negative_prompt, seed=seed, num_clips=num_clips,
                            num_inference_steps=num_inference_steps, guidance_scale=guidance_scale, width=width,
                            height=params.num_frequencies, scheduler=scheduler, output_type="latent",
-                           text_embeddings=text_embeddings, uncond_embeddings=uncond_embeddings, latents=latents)
+                           text_embeddings=text_embeddings, uncond_embeddings=uncond_embeddings, latents=latents,
+                           step_noise=step_noise)
         u8 = self._decode_u8(out["latents"])
         wave = self._u8_to_waveform(u8, converter, params.stereo, init_angles)
         return dict(images=u8, waveform=wave, latents=out["latents"], latents_unscaled=out["latents_unscaled"],
@@ -670,8 +727,9 @@ class RiffusionPipeline:
 
         Clips are grouped into loops by `text_to_audio_batch.plan_batch` (same scheduler, steps, width and side of
         guidance 1; at most `max_batch` rows), and each loop is one CFG loop whose rows keep their own guidance
-        (`DPMSolverRowsB200` / `PNDMRowsB200`).  Row r starts from `torch.randn((1, 4, 64, W/8))` drawn from a CUDA
-        generator seeded with its seed, with context [embed_text(negative or "") | embed_text(prompt)], exactly
+        (`DPMSolverRowsB200`, `PNDMRowsB200` for PNDM and DDIM, `EulerAncestralRowsB200`).  Row r starts from
+        `torch.randn((1, 4, 64, W/8))` drawn from a CUDA generator seeded with its seed (then, for Euler ancestral, one
+        draw per step from the same generator), with context [embed_text(negative or "") | embed_text(prompt)], exactly
         txt2img's draws.  After each loop, on the device: VAE decode -> uint8 image -> mel -> waveform; on the host:
         peak-normalised int16 and, with `apply_filters`, `apply_filters(compression=False)`.
 
@@ -680,7 +738,7 @@ class RiffusionPipeline:
         negative_prompt, latents_unscaled ((4, 64, W/8) fp16, the loop's output), image ((512, W, 3) uint8), waveform
         ((1, L) fp32 before normalisation), all device tensors, and segment (AudioSegment); per loop rows (clip
         indices), scheduler, num_inference_steps, width, n_unet_evals."""
-        from riffusion.scheduler_b200 import DPMSolverRowsB200, PNDMRowsB200
+        from riffusion.scheduler_b200 import SCHEDULERS, DPMSolverRowsB200, EulerAncestralRowsB200, PNDMRowsB200
         from riffusion.text_to_audio_batch import parse_batch, plan_batch
         from riffusion.util import audio_util
 
@@ -697,10 +755,16 @@ class RiffusionPipeline:
             unconds = torch.cat([self.embed_text(entries[c.entry_index].negative_prompt or "") for c in rows])
             context = self._context(None, None, len(rows), loop.cfg, texts, unconds)
             shape = (1, 4, params.num_frequencies // 8, loop.width // 8)
-            latents = torch.cat([torch.randn(shape, generator=torch.Generator(device=self.device).manual_seed(c.seed),
-                                             device=self.device, dtype=torch.float16) for c in rows]).contiguous()
-            if loop.scheduler == "PNDMScheduler":
-                sched = PNDMRowsB200(loop.num_inference_steps, [0] * len(rows), guidances, device=self._device)
+            gens = [torch.Generator(device=self.device).manual_seed(c.seed) for c in rows]
+            latents = torch.cat([torch.randn(shape, generator=g, device=self.device, dtype=torch.float16)
+                                 for g in gens]).contiguous()
+            if loop.scheduler in ("PNDMScheduler", "DDIMScheduler"):
+                sched = PNDMRowsB200(loop.num_inference_steps, [0] * len(rows), guidances, device=self._device,
+                                     scheduler=SCHEDULERS[loop.scheduler])
+            elif loop.scheduler == "EulerAncestralDiscreteScheduler":
+                sched = EulerAncestralRowsB200(loop.num_inference_steps, guidances, device=self._device)
+                self._step_noise(sched, len(sched.timesteps), latents, None, gens)
+                latents = (latents * sched.init_noise_sigma).contiguous()
             else:
                 sched = DPMSolverRowsB200(loop.num_inference_steps, guidances, device=self._device)
             latents, n_evals = self._denoise(sched, sched.timesteps, latents, context, guidances[0])
@@ -788,6 +852,7 @@ class RiffusionPipeline:
         if magic_mix and negative_prompt:
             raise ValueError("magic_mix takes no negative prompt")
         if magic_mix:
+            self._check_magic_mix_scheduler(scheduler)
             self.magic_mix_range(num_inference_steps, kmin, kmax)          # its ValueError before any device work
         if track.frame_rate != params.sample_rate:
             track = track.set_frame_rate(params.sample_rate)        # the app resamples (audio_to_audio.py:89-91)

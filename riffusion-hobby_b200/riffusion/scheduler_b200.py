@@ -1,9 +1,10 @@
 """The schedulers of the denoising loops — host-side tables + one fused device step each.
 
-`PNDMSchedulerB200` and `DPMSolverMultistepSchedulerB200` share `_ScaledLinearScheduler`: the checkpoint's ᾱ table, the
-img2img `add_noise` (`rf_axpby_f16`, with the optional inpainting mask blend) and the diffusers-style `step`.  Each keeps
-its own timestep table and multistep bookkeeping on the host; the tensor update runs in one kernel fused with the
-classifier-free-guidance combine.
+`PNDMSchedulerB200`, `DDIMSchedulerB200`, `DPMSolverMultistepSchedulerB200` and `EulerAncestralSchedulerB200` share
+`_ScaledLinearScheduler`: the checkpoint's ᾱ table, the img2img `add_noise` (`rf_axpby_f16`, with the optional inpainting
+mask blend) and the diffusers-style `step`.  Each keeps its own timestep table and multistep bookkeeping on the host; the
+tensor update runs in one kernel fused with the classifier-free-guidance combine.  DDIM is PLMS with one history term and
+runs on its kernel; Euler ancestral works in sigma space with float timesteps, scaled UNet inputs and per-step noise.
 """
 from __future__ import annotations
 
@@ -159,11 +160,42 @@ def cfg_pndm_rows_step(eps_pair: torch.Tensor, rows: torch.Tensor, ring: torch.T
     return prev
 
 
+class DDIMSchedulerB200(PNDMSchedulerB200):
+    """DDIM with eta = 0.  Restates diffusers 0.9 `DDIMScheduler(steps_offset=1, set_alpha_to_one=False,
+    clip_sample=False, beta_schedule="scaled_linear", beta_start=0.00085, beta_end=0.012)` from memory (diffusers is not
+    installable here), so it is unpinned against diffusers; the tests pin it by its first-order convergence on a model
+    whose probability-flow ODE has a closed form.
+
+    Timesteps: arange(n) * (1000 // n), reversed, + 1 (n entries, no duplicate as in PLMS).  A step from t to
+    p = t - 1000 // n is x' = sqrt(ab_p) x0 + sqrt(1 - ab_p) eps with x0 = (x - sqrt(1 - ab_t) eps) / sqrt(ab_t), and
+    ab_p = ab[0] below t = 0.  That equals PNDM's ca x - cb eps with PNDM's (ca, cb), so DDIM is PLMS with one history
+    term: `plan` always returns coef (1, 0, 0, 0), no history and no push, and the step is `rf_cfg_pndm_step_f16` (or
+    `rf_cfg_pndm_rows_step_f16` through `PNDMRowsB200`)."""
+
+    def set_timesteps(self, num_inference_steps: int, device=None) -> None:
+        self.num_inference_steps = num_inference_steps
+        ratio = self.num_train_timesteps // num_inference_steps
+        ts = (np.arange(0, num_inference_steps) * ratio).round()[::-1] + self.config["steps_offset"]
+        self.timesteps = torch.from_numpy(ts.astype(np.int64))
+        self.ets = []
+        self.counter = 0
+        self.cur_sample = None
+
+    def plan(self, timestep: int):
+        timestep = int(timestep)
+        ca, cb = self.coefficients(timestep, timestep - self.num_train_timesteps // self.num_inference_steps)
+        return (1.0, 0.0, 0.0, 0.0), [], None, False, ca, cb
+
+    def advance(self, sample, eps, push: bool, override) -> None:
+        """DDIM keeps no history: only the step count moves."""
+        self.counter += 1
+
+
 class PNDMRowsB200:
     """B independent PNDM img2img loops run as one: row r runs `PNDMSchedulerB200`'s steps over timesteps[t_starts[r]:]
     with guidance guidances[r], and all rows end on the same last timestep.  `RiffusionPipeline._denoise` drives it in
     place of a scheduler over `timesteps` = timesteps[min(t_starts):]; a row whose start has not come yet is carried
-    through unchanged.
+    through unchanged.  `scheduler` = `DDIMSchedulerB200` runs DDIM rows the same way (one history term, no push).
 
     The whole (steps x rows) table of `ROW_DTYPE` records is derived before the loop from one `PNDMSchedulerB200` per
     row (its `plan` and `advance`, run with ring-slot tokens in place of tensors) and uploaded once; each `step_cfg` is
@@ -173,11 +205,11 @@ class PNDMRowsB200:
     row that never runs a step."""
 
     def __init__(self, num_inference_steps: int, t_starts: T.Sequence[int], guidances: T.Sequence[float],
-                 device="cuda"):
+                 device="cuda", scheduler: T.Type[PNDMSchedulerB200] = PNDMSchedulerB200):
         if len(t_starts) != len(guidances) or not len(t_starts):
             raise ValueError(f"need one t_start and one guidance per row, got {len(t_starts)} and {len(guidances)}")
         guidances = rows_guidance(guidances)
-        ref = PNDMSchedulerB200()
+        ref = scheduler()
         ref.set_timesteps(num_inference_steps)
         self.all_timesteps = ref.timesteps
         n_t = len(self.all_timesteps)
@@ -189,7 +221,7 @@ class PNDMRowsB200:
         for name in ("h1", "h2", "h3", "push"):
             table[name] = -1
         for r, (t_start, g) in enumerate(zip(t_starts, guidances)):
-            s = PNDMSchedulerB200()
+            s = scheduler()
             s.set_timesteps(num_inference_steps)
             pushes = 0
             for i in range(int(t_start), n_t):
@@ -211,6 +243,9 @@ class PNDMRowsB200:
         self.ring: T.Optional[torch.Tensor] = None
         self.saved: T.Optional[torch.Tensor] = None
         self.step_index = 0
+
+    def scale_model_input(self, sample: torch.Tensor, timestep=None) -> torch.Tensor:
+        return sample
 
     def step_cfg(self, eps_pair: torch.Tensor, guidance: float, timestep: int, sample: torch.Tensor) -> torch.Tensor:
         """Guidance combine + every row's PLMS step for the next timestep of the table in one kernel.  The guidance
@@ -338,11 +373,139 @@ class DPMSolverRowsB200(DPMSolverMultistepSchedulerB200):
         return cfg_dpmpp_rows_step(eps_pair, self.guidance, sample, m1, coefs)
 
 
-SCHEDULERS = {"DPMSolverMultistepScheduler": DPMSolverMultistepSchedulerB200, "PNDMScheduler": PNDMSchedulerB200}
+def cfg_euler_a_step(eps_pair: torch.Tensor, guidance: float, guidance_rows: T.Optional[torch.Tensor],
+                     sample: torch.Tensor, noise: T.Optional[torch.Tensor], dt: float, sigma_up: float) -> torch.Tensor:
+    """Guidance combine + one Euler-ancestral update of B rows, prev = x + dt eps + sigma_up z (`rf_cfg_euler_a_step_f16`).
+    eps_pair: (2B, ...) fp16 [uncond | text]; guidance_rows: (B,) fp32, row r guided with guidance_rows[r], or None for
+    `guidance` on every row; sample: (B, ...) fp16; noise: z shaped like sample, or None for no z term.  Returns
+    prev_sample."""
+    operand(sample, "sample", torch.float16)
+    dev = sample.device
+    if sample.dim() < 1 or sample.numel() == 0:
+        raise ValueError(f"sample must hold at least one element per row, got shape {tuple(sample.shape)}")
+    B = sample.shape[0]
+    operand(eps_pair, "eps_pair", torch.float16, shape=(2 * B, *sample.shape[1:]), device=dev)
+    if guidance_rows is not None:
+        operand(guidance_rows, "guidance_rows", torch.float32, shape=(B,), device=dev)
+    if noise is not None:
+        operand(noise, "noise", torch.float16, shape=sample.shape, device=dev)
+    prev = torch.empty_like(sample)
+    _native.call("rf_cfg_euler_a_step_f16", dev, eps_pair.data_ptr(), B, sample.numel() // B, float(guidance),
+                 _native.ptr(guidance_rows), sample.data_ptr(), _native.ptr(noise), float(dt), float(sigma_up),
+                 prev.data_ptr())
+    return prev
+
+
+class EulerAncestralSchedulerB200(_ScaledLinearScheduler):
+    """Euler ancestral, in sigma space.  Restates diffusers 0.9 `EulerAncestralDiscreteScheduler` with the
+    checkpoint's scaled_linear betas 0.00085..0.012 from memory (diffusers is not installable here), so it is unpinned
+    against diffusers; the tests pin it by its weak first-order convergence on Gaussian data.
+
+    sigma(t) = ((1 - ab_t) / ab_t)^0.5 on the fp32 ab table; `init_noise_sigma` is its maximum (14.61...).  Timesteps
+    are the floats linspace(0, 999, n)[::-1] and the sampled sigmas np.interp of the table at them, then a final 0, in
+    fp32.  `scale_model_input` divides by (sigma^2 + 1)^0.5 (one `rf_axpby_f16` launch); `add_noise` is x + sigma n, with
+    no step offset for img2img.  A step from sigma to sigma' with sigma_up = (sigma'^2 (sigma^2 - sigma'^2) /
+    sigma^2)^0.5 and sigma_down = (sigma'^2 - sigma_up^2)^0.5 is x' = x + (sigma_down - sigma) eps + sigma_up z, with the
+    coefficients in fp64 from the fp32 sigmas and the tensor update fused with the guidance combine
+    (`rf_cfg_euler_a_step_f16`).
+
+    diffusers draws each step's z from the pipeline's generator inside `step`; here the loop's draws are made before
+    the loop and handed over with `set_step_noise`, so the loop runs without RNG calls.  `step_cfg` takes them in
+    order, one per step."""
+
+    def __init__(self, num_train_timesteps: int = 1000, beta_start: float = 0.00085, beta_end: float = 0.012):
+        super().__init__(num_train_timesteps, beta_start, beta_end)
+        ab = self.alphas_cumprod
+        self.sigmas_full = (((1.0 - ab) / ab) ** 0.5).numpy()
+        self.init_noise_sigma = float(self.sigmas_full.max())
+        self.config = {"num_train_timesteps": num_train_timesteps}
+        self.set_timesteps(50)
+
+    def set_timesteps(self, num_inference_steps: int, device=None) -> None:
+        self.num_inference_steps = num_inference_steps
+        ts = np.linspace(0, self.num_train_timesteps - 1, num_inference_steps, dtype=float)[::-1].copy()
+        sig = np.interp(ts, np.arange(len(self.sigmas_full)), self.sigmas_full)
+        self.sigmas = np.concatenate([sig, [0.0]]).astype(np.float32)
+        self.timesteps = torch.from_numpy(ts)
+        self.step_noise: T.Optional[torch.Tensor] = None
+        self.draws = 0
+
+    def index(self, timestep) -> int:
+        """The step index of `timestep`, found by equality as diffusers does."""
+        hits = np.flatnonzero(self.timesteps.numpy() == float(timestep))
+        if not len(hits):
+            raise ValueError(f"{float(timestep)} is not a timestep of this {self.num_inference_steps}-step schedule")
+        return int(hits[0])
+
+    def coefficients(self, timestep) -> T.Tuple[float, float]:
+        """(dt, sigma_up) of the step at `timestep`: dt = sigma_down - sigma, in fp64 from the fp32 sigmas."""
+        i = self.index(timestep)
+        s_from, s_to = float(self.sigmas[i]), float(self.sigmas[i + 1])
+        s_up = (s_to ** 2 * (s_from ** 2 - s_to ** 2) / s_from ** 2) ** 0.5
+        s_down = max(s_to ** 2 - s_up ** 2, 0.0) ** 0.5
+        return s_down - s_from, s_up
+
+    def scale_model_input(self, sample: torch.Tensor, timestep=None) -> torch.Tensor:
+        s = float(self.sigmas[self.index(timestep)])
+        x = sample.contiguous()
+        return ops.axpby(x, x, 1.0 / (s * s + 1.0) ** 0.5, 0.0)
+
+    def add_noise(self, original: torch.Tensor, noise: torch.Tensor, timestep, mask=None, blend_with=None) -> torch.Tensor:
+        s = float(self.sigmas[self.index(timestep)])
+        return ops.axpby(original.contiguous(), noise.contiguous(), 1.0, s, mask, blend_with)
+
+    def set_step_noise(self, step_noise: torch.Tensor) -> None:
+        """z of every step the loop will run, (steps, B, ...) fp16 in step order; `step_cfg` takes step_noise[k] at its
+        k-th call."""
+        self.step_noise = step_noise
+        self.draws = 0
+
+    def step_cfg(self, eps_pair: torch.Tensor, guidance: float, timestep, sample: torch.Tensor) -> torch.Tensor:
+        """Guidance combine + EulerAncestralDiscreteScheduler.step in one kernel, with the next z of `set_step_noise`.
+        eps_pair = UNet output for [uncond | text]."""
+        if self.step_noise is None or self.draws >= len(self.step_noise):
+            raise ValueError("Euler ancestral needs one noise tensor per step: call set_step_noise before the loop")
+        z = self.step_noise[self.draws]
+        self.draws += 1
+        dt, s_up = self.coefficients(timestep)
+        return self._fused_step(eps_pair.contiguous(), guidance, sample.contiguous(), z, dt, s_up)
+
+    def step(self, model_output: torch.Tensor, timestep, sample: torch.Tensor, generator=None, **kwargs):
+        """diffusers-compatible signature: the model output is already guided; z is drawn from `generator` in the
+        output's dtype, as diffusers draws it."""
+        z = torch.randn(model_output.shape, generator=generator, device=model_output.device, dtype=model_output.dtype)
+        pair = torch.cat([model_output, model_output]).contiguous()
+        dt, s_up = self.coefficients(timestep)
+        return types.SimpleNamespace(prev_sample=self._fused_step(pair, 0.0, sample.contiguous(), z, dt, s_up))
+
+    def _fused_step(self, eps_pair, guidance, sample, z, dt, s_up):
+        return cfg_euler_a_step(eps_pair, guidance, None, sample, z, dt, s_up)
+
+
+class EulerAncestralRowsB200(EulerAncestralSchedulerB200):
+    """`EulerAncestralSchedulerB200` over `num_inference_steps` for B rows that each keep their own guidance (a text to
+    audio batch): every row runs the same timesteps and sigmas and takes its own row of each step's z.  Each step is
+    one `rf_cfg_euler_a_step_f16` launch with the rows' guidance held on the device (`rows_guidance`: each row's above
+    1, else 0 for every row).  The guidance scalar the loop passes is not used."""
+
+    def __init__(self, num_inference_steps: int, guidances: T.Sequence[float], device="cuda"):
+        if not len(guidances):
+            raise ValueError("need one guidance per row, got none")
+        super().__init__()
+        self.set_timesteps(num_inference_steps)
+        self.guidance = torch.tensor(rows_guidance(guidances), dtype=torch.float32, device=device)
+
+    def _fused_step(self, eps_pair, guidance, sample, z, dt, s_up):
+        return cfg_euler_a_step(eps_pair, 0.0, self.guidance, sample, z, dt, s_up)
+
+
+# the first two keep the order of the refusal message "supported: DPMSolverMultistepScheduler, PNDMScheduler, ..."
+SCHEDULERS = {"DPMSolverMultistepScheduler": DPMSolverMultistepSchedulerB200, "PNDMScheduler": PNDMSchedulerB200,
+              "DDIMScheduler": DDIMSchedulerB200, "EulerAncestralDiscreteScheduler": EulerAncestralSchedulerB200}
 
 
 def make_scheduler(name: str):
-    """A fresh scheduler by its diffusers class name; only the two this package implements are accepted."""
+    """A fresh scheduler by its diffusers class name; only the four this package implements are accepted."""
     if name not in SCHEDULERS:
         raise ValueError(f"unsupported scheduler {name!r}; supported: {', '.join(SCHEDULERS)}")
     return SCHEDULERS[name]()

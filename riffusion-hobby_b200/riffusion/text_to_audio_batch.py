@@ -89,7 +89,8 @@ def _int(value, what: str) -> int:
 def parse_batch(data: T.Any) -> T.Tuple[T.List[ParamSet], T.List[Entry]]:
     """The parameter sets and entries of a loaded batch JSON object, with the app's defaults filled in.  Raises
     ValueError for a missing `params` or `entries`, no entries, an entry without a prompt, a width that is not a positive
-    multiple of 64, fewer than 1 step, a scheduler other than DPM-Solver++ and PNDM, or an unknown key."""
+    multiple of 64, fewer than 1 step, a scheduler other than DPM-Solver++, PNDM, DDIM and Euler ancestral, or an unknown
+    key."""
     if not isinstance(data, dict):
         raise ValueError(f"the batch must be a JSON object, got {type(data).__name__}")
     for key in ("params", "entries"):
@@ -137,7 +138,8 @@ def parse_batch(data: T.Any) -> T.Tuple[T.List[ParamSet], T.List[Entry]]:
 
 
 def n_unet_evals(scheduler: str, num_inference_steps: int) -> int:
-    """CFG evaluations of one txt2img loop: one per timestep (n for DPM-Solver++, n + 1 for PNDM)."""
+    """CFG evaluations of one txt2img loop: one per timestep (n for DPM-Solver++, DDIM and Euler ancestral, n + 1 for
+    PNDM)."""
     sched = make_scheduler(scheduler)
     sched.set_timesteps(num_inference_steps)
     return len(sched.timesteps)

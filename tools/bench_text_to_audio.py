@@ -30,7 +30,7 @@ ROOT = Path(__file__).resolve().parents[1]
 
 def n_unet_evals(scheduler: str, steps: int) -> int:
     """CFG evaluations of one txt2img call: one per timestep; PNDM's PLMS table has steps + 1 entries."""
-    if scheduler == "DPMSolverMultistepScheduler":
+    if scheduler in ("DPMSolverMultistepScheduler", "DDIMScheduler", "EulerAncestralDiscreteScheduler"):
         return steps
     if scheduler == "PNDMScheduler":
         return steps + 1
@@ -96,7 +96,9 @@ def main() -> None:
     ap.add_argument("--width", type=int, default=512, choices=[512, 768])
     ap.add_argument("--clips", type=int, default=32, help="clips per step (one CFG batch of 2 x clips)")
     ap.add_argument("--steps", type=int, default=30, help="scheduler steps")
-    ap.add_argument("--scheduler", default="DPMSolverMultistepScheduler", choices=["DPMSolverMultistepScheduler", "PNDMScheduler"])
+    ap.add_argument("--scheduler", default="DPMSolverMultistepScheduler",
+                    choices=["DPMSolverMultistepScheduler", "PNDMScheduler", "DDIMScheduler",
+                             "EulerAncestralDiscreteScheduler"])
     ap.add_argument("--reps", type=int, default=3, help="timed repetitions of the whole step")
     ap.add_argument("--unet-only", action="store_true")
     ap.add_argument("--pkg", default=str(ROOT / "riffusion-hobby_b200"))
