@@ -309,12 +309,21 @@ int rf_cfg_pndm_step_f16(const void* eps_pair, long n, float guidance, const voi
  * The arithmetic is rf_cfg_pndm_step_f16's term for term: a table whose rows all hold one step gives its bits. */
 #define RF_PNDM_ROW_BASE_SAVED 1
 #define RF_PNDM_ROW_SAVE 2
+#define RF_PNDM_ROW_MASK 4
 typedef struct rf_pndm_row {
     float guidance, c0, c1, c2, c3, ca, cb;
     int32_t active, h1, h2, h3, push, flags;
 } rf_pndm_row;
 int rf_cfg_pndm_rows_step_f16(const void* eps_pair, int B, long m, const rf_pndm_row* d_rows, void* ring, void* saved,
                               const void* sample, void* prev_sample, void* stream);
+/* rf_cfg_pndm_rows_step_f16 with a per-row inpainting blend: an active row whose flags hold RF_PNDM_ROW_MASK forms its
+ * stepped value p (rounded to fp16) and stores (a init + b noise) mask + p (1 - mask), rounded once, which is the bits of
+ * rf_cfg_pndm_rows_step_f16 followed by rf_axpby_f16(init, noise, a, b, mask, p).  init (the row's clean latents),
+ * noise (its slerped noise) and mask: fp16 [B][m], read only for the rows that blend; a = sqrt(ab_t), b = sqrt(1 - ab_t)
+ * at the loop's current timestep, shared by every row.  Rows without the flag give rf_cfg_pndm_rows_step_f16's bits. */
+int rf_cfg_pndm_rows_mask_step_f16(const void* eps_pair, int B, long m, const rf_pndm_row* d_rows, void* ring,
+                                   void* saved, const void* sample, const void* init, const void* noise,
+                                   const void* mask, float a, float b, void* prev_sample, void* stream);
 /* classifier-free guidance + DPM-Solver++ (2M, midpoint) update on n = elements of ONE batch half:
  *   eps = eps_u + g (eps_t - eps_u) (fp16, as rf_cfg_pndm_step_f16); x0 = (x - sigma_s0 eps) / alpha_s0;
  *   prev = c_x x + c_0 x0 + c_1 (x0 - m1), the last term only when m1 (the previous step's x0) is given.

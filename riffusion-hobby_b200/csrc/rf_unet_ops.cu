@@ -691,15 +691,26 @@ __global__ void k_cfg_pndm_step(const __half* __restrict__ eps_pair, size_t n, f
 // its own timestep and keeps its own guidance).  blockIdx.y = row; the row's record is read once per thread.  Slots
 // outside 0..3 count as absent, so a malformed record cannot index outside the ring.  Each element's ring / saved
 // reads come before its writes in the same thread, so no slot aliasing can race.
+// kMask: an active row whose record has RF_PNDM_ROW_MASK then applies the inpainting blend of riffuse to its stepped
+// value p (already rounded to fp16): prev = (a init + b noise) m + p (1 - m), rounded once.  That is k_axpby with
+// x = init, nz = noise, z = p.  nvcc compiles k_axpby's `a * x + b * n` to FMUL(b, n) then FFMA(a, x, .), and
+// `v * m + z * (1 - m)` to FADD(1 - m), FMUL(z, 1 - m) then FFMA(v, m, .) (cuobjdump -sass, sm_90a, CUDA 12.9); the
+// same operations are spelled out here with explicit roundings, so a masked row gives the bits of the rows step followed
+// by rf_axpby_f16 whatever either kernel's contraction.  Rows without the flag and inactive rows never read init /
+// noise / mask.  kMask = false is the plain rows step.
+template <bool kMask>
 __global__ void k_cfg_pndm_rows_step(const __half* __restrict__ eps_pair, int B, size_t m,
                                      const rf_pndm_row* __restrict__ rows, __half* ring, __half* saved,
-                                     const __half* __restrict__ sample, __half* __restrict__ prev_sample) {
+                                     const __half* __restrict__ sample, __half* __restrict__ prev_sample,
+                                     const __half* __restrict__ init, const __half* __restrict__ noise,
+                                     const __half* __restrict__ mask, float a, float b) {
     const int r = blockIdx.y;
     const rf_pndm_row rec = rows[r];
     const size_t row0 = static_cast<size_t>(r) * m, plane = static_cast<size_t>(B) * m;
     const bool has1 = static_cast<unsigned>(rec.h1) < 4u, has2 = static_cast<unsigned>(rec.h2) < 4u,
                has3 = static_cast<unsigned>(rec.h3) < 4u, push = static_cast<unsigned>(rec.push) < 4u;
     const bool from_saved = rec.flags & RF_PNDM_ROW_BASE_SAVED, save = rec.flags & RF_PNDM_ROW_SAVE;
+    const bool blend = kMask && (rec.flags & RF_PNDM_ROW_MASK);
     for (size_t k = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x; k < m;
          k += static_cast<size_t>(gridDim.x) * blockDim.x) {
         const size_t i = row0 + k;
@@ -719,7 +730,14 @@ __global__ void k_cfg_pndm_rows_step(const __half* __restrict__ eps_pair, int B,
         const float base = __half2float(from_saved ? saved[i] : x);
         if (push) ring[rec.push * plane + i] = e0;
         if (save) saved[i] = x;
-        prev_sample[i] = __float2half_rn(__fmaf_rn(rec.ca, base, -__fmul_rn(rec.cb, e)));
+        const __half p = __float2half_rn(__fmaf_rn(rec.ca, base, -__fmul_rn(rec.cb, e)));
+        if (kMask && blend) {
+            const float mk = __half2float(mask[i]);
+            const float v = __fmaf_rn(a, __half2float(init[i]), __fmul_rn(b, __half2float(noise[i])));
+            prev_sample[i] = __float2half_rn(__fmaf_rn(v, mk, __fmul_rn(__half2float(p), __fsub_rn(1.f, mk))));
+        } else {
+            prev_sample[i] = p;
+        }
     }
 }
 
@@ -1155,10 +1173,29 @@ extern "C" int rf_cfg_pndm_rows_step_f16(const void* eps_pair, int B, long m, co
     const size_t per_row = static_cast<size_t>(m);
     // the grid-stride budget of the whole batch, split evenly over the rows
     const unsigned bx = std::max(1u, grid_for(per_row * B, 256) / static_cast<unsigned>(B));
-    k_cfg_pndm_rows_step<<<dim3(bx, static_cast<unsigned>(B)), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+    k_cfg_pndm_rows_step<false><<<dim3(bx, static_cast<unsigned>(B)), 256, 0, static_cast<cudaStream_t>(stream)>>>(
         static_cast<const __half*>(eps_pair), B, per_row, d_rows, static_cast<__half*>(ring),
-        static_cast<__half*>(saved), static_cast<const __half*>(sample), static_cast<__half*>(prev_sample));
+        static_cast<__half*>(saved), static_cast<const __half*>(sample), static_cast<__half*>(prev_sample), nullptr,
+        nullptr, nullptr, 0.f, 0.f);
     RF_CUDA_LAUNCH_CHECK("k_cfg_pndm_rows_step");
+    return RF_OK;
+}
+
+extern "C" int rf_cfg_pndm_rows_mask_step_f16(const void* eps_pair, int B, long m, const rf_pndm_row* d_rows,
+                                              void* ring, void* saved, const void* sample, const void* init,
+                                              const void* noise, const void* mask, float a, float b, void* prev_sample,
+                                              void* stream) {
+    if (!eps_pair || !d_rows || !ring || !saved || !sample || !init || !noise || !mask || !prev_sample || B <= 0 ||
+        B > 65535 || m <= 0)
+        return rf_fail(RF_ERR_INVALID, "rf_cfg_pndm_rows_mask_step_f16: bad argument");
+    const size_t per_row = static_cast<size_t>(m);
+    // the grid-stride budget of the whole batch, split evenly over the rows (as rf_cfg_pndm_rows_step_f16)
+    const unsigned bx = std::max(1u, grid_for(per_row * B, 256) / static_cast<unsigned>(B));
+    k_cfg_pndm_rows_step<true><<<dim3(bx, static_cast<unsigned>(B)), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+        static_cast<const __half*>(eps_pair), B, per_row, d_rows, static_cast<__half*>(ring),
+        static_cast<__half*>(saved), static_cast<const __half*>(sample), static_cast<__half*>(prev_sample),
+        static_cast<const __half*>(init), static_cast<const __half*>(noise), static_cast<const __half*>(mask), a, b);
+    RF_CUDA_LAUNCH_CHECK("k_cfg_pndm_rows_mask_step");
     return RF_OK;
 }
 

@@ -122,6 +122,9 @@ SIGNATURES = {
                                        C.c_void_p]),
     "rf_cfg_pndm_rows_step_f16": (C.c_int, [C.c_void_p, C.c_int, C.c_long, C.c_void_p, C.c_void_p, C.c_void_p,
                                             C.c_void_p, C.c_void_p, C.c_void_p]),
+    "rf_cfg_pndm_rows_mask_step_f16": (C.c_int, [C.c_void_p, C.c_int, C.c_long, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                 C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_float, C.c_float,
+                                                 C.c_void_p, C.c_void_p]),
     "rf_cfg_dpmpp_step_f16": (C.c_int, [C.c_void_p, C.c_long, C.c_float, C.c_void_p, C.c_void_p, C.c_float, C.c_float,
                                         C.c_float, C.c_float, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p]),
     "rf_cfg_dpmpp_rows_step_f16": (C.c_int, [C.c_void_p, C.c_int, C.c_long, C.c_void_p, C.c_void_p, C.c_void_p,

@@ -248,7 +248,6 @@ class RiffusionPipeline:
         ends' guidance lies on different sides of 1, or when the seed image's height (rounded down to a multiple of 32)
         is not params.num_frequencies.  Returns dict(segment, images ((n, H, W, 3) uint8 device
         tensor), waveform ((n, channels, L) fp32 before normalisation), alphas, requests, n_unet_evals (per loop))."""
-        from riffusion.scheduler_b200 import PNDMRowsB200
         from riffusion.util import audio_util
 
         n = num_interpolation_steps
@@ -276,19 +275,11 @@ class RiffusionPipeline:
         u8s, waves, n_evals = [], [], []
         for lo in range(0, n, max_batch):
             idx = list(range(lo, min(n, lo + max_batch)))
-            texts, lats, noise = self._prepare_requests(requests, idx, self.embed_text_weighted, images, None)
-            lats = lats.to(device=self._device, dtype=torch.float16).contiguous()
-            noise = noise.to(self._device, torch.float16).contiguous()
-            latents = torch.cat([sched.add_noise(lats[j:j + 1], noise[j:j + 1], int(sched.timesteps[-steps[i][0]]))
-                                 for j, i in enumerate(idx)])
-            rows = PNDMRowsB200(num_inference_steps, [steps[i][1] for i in idx], [guidances[i] for i in idx],
-                                device=self._device)
-            context = self._context(None, None, len(idx), guidances[lo] > 1.0, texts, None)
-            latents, evals = self._denoise(rows, rows.timesteps, latents, context, guidances[lo])
-            n_evals.append(evals)
-            u8 = self._decode_u8((1.0 / VAE_SCALE) * latents)
             angles = None if init_angles is None else init_angles[lo:lo + len(idx)]
-            waves.append(self._u8_to_waveform(u8, converter, params.stereo, angles))
+            u8, wave, evals = self._rows_loop(requests, idx, images, sched, [steps[i] for i in idx],
+                                              [guidances[i] for i in idx], converter, params.stereo, angles)
+            n_evals.append(evals)
+            waves.append(wave)
             u8s.append(u8)
         waveform = torch.cat(waves)
         segments = []
@@ -297,6 +288,145 @@ class RiffusionPipeline:
             segments.append(audio_util.apply_filters(seg, compression=False) if apply_filters else seg)
         return dict(segment=audio_util.stitch_segments(segments, crossfade_s=0), images=torch.cat(u8s),
                     waveform=waveform, alphas=alphas, requests=requests, n_unet_evals=n_evals)
+
+    def _rows_loop(self, requests: T.Sequence[InferenceInput], idx: T.Sequence[int],
+                   images: T.Sequence[Image.Image], sched, starts: T.Sequence[T.Tuple[int, int]],
+                   guidances: T.Sequence[float], converter, stereo: bool, angles: T.Optional[torch.Tensor], *,
+                   masks: T.Optional[T.Sequence[T.Optional[torch.Tensor]]] = None,
+                   n_fill: int = 0, waveform: bool = True) -> T.Tuple[torch.Tensor, T.Optional[torch.Tensor], int]:
+        """The loop body of `interpolation` and `riffuse_requests`: requests[i], i in idx, as the rows of one CFG loop.
+        Row k draws what `riffuse` draws for its request (`_prepare_requests`), is noised at
+        sched.timesteps[-init_timestep] with (init_timestep, t_start) = starts[k], and joins a `PNDMRowsB200` loop of
+        type(sched) at its own t_start with guidances[k].  masks[k], a (1, 4, h, w) fp16 device mask or None, gives row k
+        riffuse's inpainting blend inside the step kernel.  `n_fill` filler rows, copies of the last row that start at
+        len(timesteps) and so never step, pad the loop's batch; they are dropped before the VAE.  After the loop, on the
+        device: VAE decode -> uint8 image -> waveform (`angles` fixes Griffin-Lim's initial phases; None with
+        `waveform=False`).  Returns (uint8 images, waveform, UNet evaluations)."""
+        from riffusion.scheduler_b200 import PNDMRowsB200
+
+        texts, lats, noise = self._prepare_requests(requests, idx, self.embed_text_weighted, images, None)
+        lats = lats.to(device=self._device, dtype=torch.float16).contiguous()
+        noise = noise.to(self._device, torch.float16).contiguous()
+        latents = torch.cat([sched.add_noise(lats[k:k + 1], noise[k:k + 1], int(sched.timesteps[-starts[k][0]]))
+                             for k in range(len(idx))])
+        if n_fill:
+            def pad(t: torch.Tensor) -> torch.Tensor:
+                return torch.cat([t, t[-1:].expand(n_fill, *t.shape[1:])]).contiguous()
+
+            texts, lats, noise, latents = pad(texts), pad(lats), pad(noise), pad(latents)
+        masks = [None] * len(idx) if masks is None else list(masks)
+        t_starts = [s[1] for s in starts] + [len(sched.timesteps)] * n_fill
+        rows = PNDMRowsB200(sched.num_inference_steps, t_starts, list(guidances) + [guidances[-1]] * n_fill,
+                            device=self._device, scheduler=type(sched),
+                            masked=[m is not None for m in masks] + [False] * n_fill)
+        if rows.masked:
+            blank = torch.zeros_like(lats[:1])
+            mask = torch.cat([blank if m is None else m.to(device=self._device, dtype=torch.float16).expand_as(blank)
+                              for m in masks] + [blank] * n_fill).contiguous()
+            rows.set_mask_inputs(init=lats, noise=noise, mask=mask)
+        context = self._context(None, None, len(t_starts), guidances[0] > 1.0, texts, None)
+        latents, evals = self._denoise(rows, rows.timesteps, latents, context, guidances[0])
+        u8 = self._decode_u8((1.0 / VAE_SCALE) * latents[:len(idx)])
+        wave = self._u8_to_waveform(u8, converter, stereo, angles) if waveform else None
+        return u8, wave, evals
+
+    def context_error(self, inputs: InferenceInput) -> T.Optional[str]:
+        """Why `riffuse` cannot build this request's CFG context, or None.  Its weighted prompts embed to 77 k tokens:
+        the start and end embeddings must have one length for the lerp, and with guidance above 1 that length must be
+        the unconditional embedding's (77).  `riffuse` (as the reference) fails inside torch otherwise."""
+        e0 = self.embed_text_weighted(inputs.start.prompt)
+        e1 = self.embed_text_weighted(inputs.end.prompt)
+        if e0.shape != e1.shape:
+            return f"the start and end prompts embed to {e0.shape[1]} and {e1.shape[1]} tokens"
+        guidance = inputs.start.guidance * (1.0 - inputs.alpha) + inputs.end.guidance * inputs.alpha
+        n_uncond = self.embed_text("").shape[1]
+        if guidance > 1.0 and e0.shape[1] != n_uncond:
+            return (f"the prompts embed to {e0.shape[1]} tokens; guidance {guidance} needs {n_uncond}, the length of the "
+                    "unconditional embedding")
+        return None
+
+    @staticmethod
+    def request_loops(keys: T.Sequence[T.Hashable], max_batch: int) -> T.List[T.Tuple[T.List[int], int]]:
+        """The loops of `riffuse_requests` for requests with these group keys: one group per distinct key, in order of
+        first arrival, requests in arrival order, cut into chunks of at most `max_batch`.  Each chunk runs at a batch of
+        its row count rounded up to a power of two, at most `max_batch`, so a pipeline captures at most
+        log2(max_batch) + 2 CUDA graphs per (latent shape, context shape).  Returns [(request indices, batch)]."""
+        if max_batch < 1:
+            raise ValueError("max_batch must be at least 1")
+        groups: T.Dict[T.Hashable, T.List[int]] = {}
+        for i, key in enumerate(keys):
+            groups.setdefault(key, []).append(i)
+        loops = []
+        for idx in groups.values():
+            for lo in range(0, len(idx), max_batch):
+                chunk = idx[lo:lo + max_batch]
+                loops.append((chunk, min(max_batch, 1 << (len(chunk) - 1).bit_length())))
+        return loops
+
+    @torch.no_grad()
+    def riffuse_requests(self, inputs: T.Sequence[InferenceInput], init_images: T.Sequence[Image.Image],
+                         mask_images: T.Sequence[T.Optional[Image.Image]], *, max_batch: int = 16,
+                         init_angles: T.Optional[T.Sequence[torch.Tensor]] = None,
+                         waveform: bool = True) -> T.List[T.Dict[str, T.Any]]:
+        """`riffuse` of many requests, each with its own seed image and optional mask, in as few CFG loops as their
+        shapes allow: the model server's batch entry point.
+
+        One loop per group of (num_inference_steps, latent shape, context length, guidance > 1), requests in arrival
+        order, chunked at `max_batch` (`request_loops`).  In its loop each request is a row that draws what `riffuse`
+        draws for it, joins at its own `_img2img_steps` start with its own lerped guidance and, with a mask, applies
+        riffuse's inpainting blend after each of its steps (`PNDMRowsB200` with `masked`).  A chunk's batch is its row
+        count rounded up to a power of two (at most `max_batch`); the filler rows never step and are dropped.  After
+        each loop, on the device: VAE decode -> uint8 image -> mel -> waveform, mono 0-10 kHz; `init_angles`, one
+        (1, n_fft/2 + 1, frames) complex64 tensor per request, fixes Griffin-Lim's initial phases; `waveform=False`
+        skips the audio (the results' waveform is None).  The pipeline's scheduler must be PNDM or DDIM.
+
+        Raises ValueError before any device work for another scheduler, lists of other lengths, max_batch below 1, or
+        a mask whose size differs from its seed image, and before any loop for prompts whose context `riffuse` cannot
+        build (`context_error`), naming the request.  Returns per request dict(image ((H, W, 3) uint8 device tensor),
+        waveform ((1, L) fp32 before normalisation), loop (the loop's index), n_unet_evals (its loop's), filler_rows
+        (its loop's))."""
+        n = len(inputs)
+        if type(self.scheduler) not in (PNDMSchedulerB200, DDIMSchedulerB200):
+            raise ValueError(f"riffuse_requests runs PNDM or DDIM rows, not {type(self.scheduler).__name__}")
+        if len(init_images) != n or len(mask_images) != n or (init_angles is not None and len(init_angles) != n):
+            raise ValueError(f"need one seed image, one mask (or None) and one set of angles per request: {n} requests, "
+                             f"{len(init_images)} images, {len(mask_images)} masks")
+        if max_batch < 1:
+            raise ValueError("max_batch must be at least 1")
+        for i, (img, mask) in enumerate(zip(init_images, mask_images)):
+            if mask is not None and mask.size != img.size:
+                raise ValueError(f"request {i}: mask image is {mask.size[0]}x{mask.size[1]}, its seed image "
+                                 f"{img.size[0]}x{img.size[1]}")
+        for i, r in enumerate(inputs):
+            error = self.context_error(r)
+            if error is not None:
+                raise ValueError(f"request {i}: {error}")
+        sched_cls = type(self.scheduler)
+        strengths = [(1 - r.alpha) * r.start.denoising + r.alpha * r.end.denoising for r in inputs]    # as riffuse
+        guidances = [r.start.guidance * (1.0 - r.alpha) + r.end.guidance * r.alpha for r in inputs]
+        keys = []
+        for r, img, g in zip(inputs, init_images, guidances):
+            w, h = img.size
+            ctx = self.embed_text_weighted(r.start.prompt).shape[1]
+            keys.append((r.num_inference_steps, ((h - h % 32) // 8, (w - w % 32) // 8), ctx, g > 1.0))
+        scale = 2 ** (len(self.vae.config.block_out_channels) - 1)
+        masks = [None if m is None else preprocess_mask(m, scale_factor=scale).to(device=self.device, dtype=torch.float16)
+                 for m in mask_images]
+        converter = self._converter(DEFAULT_PARAMS, None) if waveform else None
+        results: T.List[T.Optional[T.Dict[str, T.Any]]] = [None] * n
+        for loop, (idx, batch) in enumerate(self.request_loops(keys, max_batch)):
+            sched = sched_cls()
+            sched.set_timesteps(inputs[idx[0]].num_inference_steps)
+            starts = [self._img2img_steps(sched, sched.num_inference_steps, strengths[i]) for i in idx]
+            angles = None if init_angles is None else torch.stack([init_angles[i] for i in idx])
+            u8, wave, evals = self._rows_loop(inputs, idx, init_images, sched, starts, [guidances[i] for i in idx],
+                                              converter, DEFAULT_PARAMS.stereo, angles,
+                                              masks=[masks[i] for i in idx], n_fill=batch - len(idx),
+                                              waveform=waveform)
+            for k, i in enumerate(idx):
+                results[i] = dict(image=u8[k], waveform=None if wave is None else wave[k], loop=loop, n_unet_evals=evals,
+                                  filler_rows=batch - len(idx))
+        return results  # type: ignore[return-value]
 
     def encode_image(self, init_image: Image.Image, generator: torch.Generator) -> torch.Tensor:
         """preprocess + VAE posterior sample * 0.18215 (:252-264).  The (mean, logvar) moments only depend on the

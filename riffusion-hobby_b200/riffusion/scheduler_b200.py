@@ -127,7 +127,7 @@ class PNDMSchedulerB200(_ScaledLinearScheduler):
 
 ROW_DTYPE = np.dtype([(name, np.float32) for name in ("guidance", "c0", "c1", "c2", "c3", "ca", "cb")] +
                      [(name, np.int32) for name in ("active", "h1", "h2", "h3", "push", "flags")])   # rf_pndm_row
-ROW_BASE_SAVED, ROW_SAVE = 1, 2           # RF_PNDM_ROW_BASE_SAVED, RF_PNDM_ROW_SAVE
+ROW_BASE_SAVED, ROW_SAVE, ROW_MASK = 1, 2, 4     # RF_PNDM_ROW_BASE_SAVED, RF_PNDM_ROW_SAVE, RF_PNDM_ROW_MASK
 _SAVED = "saved"                          # the token `advance` keeps as a row's first sample
 
 
@@ -157,6 +157,31 @@ def cfg_pndm_rows_step(eps_pair: torch.Tensor, rows: torch.Tensor, ring: torch.T
     prev = torch.empty_like(sample)
     _native.call("rf_cfg_pndm_rows_step_f16", dev, eps_pair.data_ptr(), B, sample.numel() // B, rows.data_ptr(),
                  ring.data_ptr(), saved.data_ptr(), sample.data_ptr(), prev.data_ptr())
+    return prev
+
+
+def cfg_pndm_rows_mask_step(eps_pair: torch.Tensor, rows: torch.Tensor, ring: torch.Tensor, saved: torch.Tensor,
+                            sample: torch.Tensor, init: torch.Tensor, noise: torch.Tensor, mask: torch.Tensor, a: float,
+                            b: float) -> torch.Tensor:
+    """`cfg_pndm_rows_step` with the inpainting blend of the rows whose record holds `ROW_MASK`
+    (`rf_cfg_pndm_rows_mask_step_f16`): such a row stores (a init + b noise) mask + p (1 - mask), p its stepped value in
+    fp16.  init, noise, mask: (B, ...) fp16 shaped like sample, read only for those rows; a = sqrt(ab_t), b = sqrt(1 -
+    ab_t) at the step's timestep.  Returns prev_sample."""
+    operand(sample, "sample", torch.float16)
+    dev = sample.device
+    if sample.dim() < 1 or sample.numel() == 0:
+        raise ValueError(f"sample must hold at least one element per row, got shape {tuple(sample.shape)}")
+    B = sample.shape[0]
+    operand(eps_pair, "eps_pair", torch.float16, shape=(2 * B, *sample.shape[1:]), device=dev)
+    operand(rows, "rows", torch.int32, shape=(B, ROW_DTYPE.itemsize // 4), device=dev)
+    operand(ring, "ring", torch.float16, shape=(4, *sample.shape), device=dev)
+    operand(saved, "saved", torch.float16, shape=sample.shape, device=dev)
+    for t, name in ((init, "init"), (noise, "noise"), (mask, "mask")):
+        operand(t, name, torch.float16, shape=sample.shape, device=dev)
+    prev = torch.empty_like(sample)
+    _native.call("rf_cfg_pndm_rows_mask_step_f16", dev, eps_pair.data_ptr(), B, sample.numel() // B, rows.data_ptr(),
+                 ring.data_ptr(), saved.data_ptr(), sample.data_ptr(), init.data_ptr(), noise.data_ptr(),
+                 mask.data_ptr(), float(a), float(b), prev.data_ptr())
     return prev
 
 
@@ -196,6 +221,9 @@ class PNDMRowsB200:
     with guidance guidances[r], and all rows end on the same last timestep.  `RiffusionPipeline._denoise` drives it in
     place of a scheduler over `timesteps` = timesteps[min(t_starts):]; a row whose start has not come yet is carried
     through unchanged.  `scheduler` = `DDIMSchedulerB200` runs DDIM rows the same way (one history term, no push).
+    With `masked`, row r (masked[r] true) applies riffuse's inpainting blend after each of its steps inside the step
+    kernel (`ROW_MASK` in its records, `rf_cfg_pndm_rows_mask_step_f16`): `set_mask_inputs` hands over the rows' clean
+    latents, noise and masks, and the blend is at the ᾱ of the loop's timestep, as `add_noise` takes it.
 
     The whole (steps x rows) table of `ROW_DTYPE` records is derived before the loop from one `PNDMSchedulerB200` per
     row (its `plan` and `advance`, run with ring-slot tokens in place of tensors) and uploaded once; each `step_cfg` is
@@ -205,9 +233,13 @@ class PNDMRowsB200:
     row that never runs a step."""
 
     def __init__(self, num_inference_steps: int, t_starts: T.Sequence[int], guidances: T.Sequence[float],
-                 device="cuda", scheduler: T.Type[PNDMSchedulerB200] = PNDMSchedulerB200):
+                 device="cuda", scheduler: T.Type[PNDMSchedulerB200] = PNDMSchedulerB200,
+                 masked: T.Optional[T.Sequence[bool]] = None):
         if len(t_starts) != len(guidances) or not len(t_starts):
             raise ValueError(f"need one t_start and one guidance per row, got {len(t_starts)} and {len(guidances)}")
+        masked = [False] * len(t_starts) if masked is None else [bool(v) for v in masked]
+        if len(masked) != len(t_starts):
+            raise ValueError(f"need one masked flag per row, got {len(masked)} for {len(t_starts)} rows")
         guidances = rows_guidance(guidances)
         ref = scheduler()
         ref.set_timesteps(num_inference_steps)
@@ -220,7 +252,7 @@ class PNDMRowsB200:
         table = np.zeros((n_t - self.t0, len(t_starts)), dtype=ROW_DTYPE)
         for name in ("h1", "h2", "h3", "push"):
             table[name] = -1
-        for r, (t_start, g) in enumerate(zip(t_starts, guidances)):
+        for r, (t_start, g, blend) in enumerate(zip(t_starts, guidances, masked)):
             s = scheduler()
             s.set_timesteps(num_inference_steps)
             pushes = 0
@@ -235,7 +267,8 @@ class PNDMRowsB200:
                     rec[name] = slot
                 slot = pushes % 4 if push else -1
                 rec["push"] = slot
-                rec["flags"] = (ROW_SAVE if s.counter == 0 else 0) | (ROW_BASE_SAVED if override == _SAVED else 0)
+                rec["flags"] = ((ROW_SAVE if s.counter == 0 else 0) | (ROW_BASE_SAVED if override == _SAVED else 0) |
+                                (ROW_MASK if blend else 0))
                 s.advance(_SAVED, slot, push, override)
                 pushes += push
         self.table = table
@@ -243,6 +276,16 @@ class PNDMRowsB200:
         self.ring: T.Optional[torch.Tensor] = None
         self.saved: T.Optional[torch.Tensor] = None
         self.step_index = 0
+        self.masked = any(masked)
+        self.alphas_cumprod = ref.alphas_cumprod
+        self.mask_inputs: T.Optional[T.Tuple[torch.Tensor, torch.Tensor, torch.Tensor]] = None
+
+    def set_mask_inputs(self, *, init: torch.Tensor, noise: torch.Tensor, mask: torch.Tensor) -> None:
+        """The masked rows' blend inputs, each (B, 4, h, w) fp16 on the device: clean latents, slerped noise and mask.
+        The rows without a mask are never read."""
+        if not self.masked:
+            raise ValueError("no row of this table is masked")
+        self.mask_inputs = (init, noise, mask)
 
     def scale_model_input(self, sample: torch.Tensor, timestep=None) -> torch.Tensor:
         return sample
@@ -256,7 +299,14 @@ class PNDMRowsB200:
         if self.ring is None:
             self.ring = torch.empty((4, *sample.shape), dtype=sample.dtype, device=sample.device)
             self.saved = torch.empty_like(sample)
-        prev = cfg_pndm_rows_step(eps_pair.contiguous(), self.rows[j], self.ring, self.saved, sample.contiguous())
+        if self.masked:
+            if self.mask_inputs is None:
+                raise ValueError("masked rows need their blend inputs: call set_mask_inputs before the loop")
+            ab = float(self.alphas_cumprod[int(timestep)])
+            prev = cfg_pndm_rows_mask_step(eps_pair.contiguous(), self.rows[j], self.ring, self.saved,
+                                           sample.contiguous(), *self.mask_inputs, ab ** 0.5, (1.0 - ab) ** 0.5)
+        else:
+            prev = cfg_pndm_rows_step(eps_pair.contiguous(), self.rows[j], self.ring, self.saved, sample.contiguous())
         self.step_index += 1
         return prev
 
