@@ -5,7 +5,8 @@
 // TMA engine: one 4-D box load per filter tap with out-of-bounds zero fill supplying the padding).
 //
 // CTA = one 128 x BN output tile at a time.  Warp roles: warps 0-7 = two consumer warpgroups (rows 0-63 / 64-127 of the
-// tile: wgmma m64nBNk16 with both operands in shared memory, then the epilogue), warp 8 = TMA producer (one thread).
+// tile: wgmma m64nBNk16 with both operands in shared memory), warp 8 = TMA producer (one thread), warps 9-15 = epilogue
+// (the finished tile arrives through an fp32 staging tile while the consumers already run the next tile's MMAs).
 // K is streamed in 64-element (128-byte, SWIZZLE_128B) slabs through a STAGES-deep mbarrier ring.
 //
 // Reference arithmetic this replaces (diffusers 0.9 modules reached from
@@ -30,7 +31,13 @@ namespace {
 constexpr int BM = 128;
 constexpr int BK = 64;
 constexpr int A_TILE_BYTES = BM * BK * 2;  // 16 KB
-constexpr int GEMM_THREADS = 256 + 32;     // two consumer warpgroups + one producer warp
+// two consumer warpgroups + one producer warp + seven epilogue warps.  16 warps leave each SM sub-partition (16 K
+// registers, 4 of the warps) 128 registers per thread; an eighth epilogue warp would put 5 warps on one sub-partition and
+// leave 96, below what the BN 160 consumers need.  Four epilogue warps were too few: the GEGLU epilogue then outlasted
+// its 5-slab mainloop (DESIGN 3b).
+constexpr int EPI_THREAD0 = 256 + 32;          // first epilogue thread
+constexpr int EPI_THREADS = 224;
+constexpr int GEMM_THREADS = EPI_THREAD0 + EPI_THREADS;
 constexpr int STAGE_PAD = 4;               // fp32 staging row pitch BN + 4: row-per-thread float4 reads are conflict free
 
 __host__ __device__ constexpr int stage_bytes(int BN) { return BM * (BN + STAGE_PAD) * 4; }
@@ -101,14 +108,16 @@ __device__ __forceinline__ float gelu_erf_fast(float g) {
     return g * (g < 0.f ? (t < 4.0f ? h : 0.f) : 1.f - h);
 }
 
-__device__ __forceinline__ void named_bar_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
-
 // Persistent kernel: grid = min(#tiles, #SMs) CTAs, each walking work units t = blockIdx.x, +gridDim.x, ...
-//   warp 8:    TMA producer — streams the K slabs of all its units through one STAGES-deep ring (phases run across units)
-//   warps 0-7: two consumer warpgroups — wgmma into register accumulators, releasing each ring stage as soon as the MMAs
-//              that read it have completed; then the accumulators go through an fp32 staging tile in shared memory to a
-//              row-per-thread epilogue (bias / activation / residual / GEGLU / split-K partials).  The producer keeps
-//              filling the ring for the next unit while the epilogue runs.
+//   warp 8:     TMA producer — streams the K slabs of all its units through one STAGES-deep ring (phases run across units)
+//   warps 0-7:  two consumer warpgroups — wgmma into register accumulators, releasing each ring stage as soon as the MMAs
+//               that read it have completed; then they wait until the staging tile is free (stg_empty), write the
+//               accumulators to it, arrive on stg_full and go straight on to the next unit's MMAs
+//   warps 9-15: epilogue — walk the same units; per unit they wait on stg_full and run the epilogue (bias / activation /
+//               residual / GEGLU / split-K partials) over the tile's 32-column row runs from the staging tile, arriving
+//               on stg_empty after their last staging read.  So a tile's global stores and side-input loads overlap the
+//               next tile's mainloop instead of idling the tensor pipe, which matters most where a tile has few K slabs
+//               (K = 320: five).
 // Tile order: n fastest, then m, then batch, so CTAs running at the same time share activation rows in L2.
 //
 // BRES = true (K <= BRES_KB slabs, non-batched): B-stationary.  A CTA stays on ONE column block, loads all K slabs of its
@@ -129,6 +138,8 @@ k_tc_gemm(const __grid_constant__ CUtensorMap mapA0, const __grid_constant__ CUt
     uint64_t* full = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(stg) + stage_bytes(BN));
     uint64_t* empty = full + STAGES;
     uint64_t* b_full = empty + STAGES;          // BRES: the resident B tile has landed
+    uint64_t* stg_full = b_full + 1;            // the consumers have written a unit's accumulators to the staging tile
+    uint64_t* stg_empty = stg_full + 1;         // the epilogue warps are done reading it
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int tiles_mn = p.tiles_n * p.tiles_m;
@@ -145,6 +156,8 @@ k_tc_gemm(const __grid_constant__ CUtensorMap mapA0, const __grid_constant__ CUt
             tc::mbar_init(&empty[i], 256);      // every consumer thread arrives once it is done with the stage
         }
         tc::mbar_init(b_full, 1);
+        tc::mbar_init(stg_full, 256);
+        tc::mbar_init(stg_empty, EPI_THREADS);
         tc::fence_barrier_init();
     }
     if (warp == 8 && lane == 0) {
@@ -202,90 +215,104 @@ k_tc_gemm(const __grid_constant__ CUtensorMap mapA0, const __grid_constant__ CUt
         return;
     }
 
-    // ---------------------------------------------------------------- consumers (threads 0-255)
-    const int wg = warp >> 2;                    // rows [64 wg, +64) of the tile
-    const int frag_row = wg * 64 + (warp & 3) * 16 + (lane >> 2), frag_col = 2 * (lane & 3);
-    const int row = threadIdx.x & 127;           // epilogue: one tile row per thread, two threads per row
-    const int half_id = threadIdx.x >> 7;
+    if (warp < 8) {
+        // ------------------------------------------------------------ consumers (threads 0-255)
+        const int wg = warp >> 2;                    // rows [64 wg, +64) of the tile
+        const int frag_row = wg * 64 + (warp & 3) * 16 + (lane >> 2), frag_col = 2 * (lane & 3);
+        if constexpr (BRES) tc::mbar_wait(b_full, 0);
+        int it = 0, done = 0;                        // units done: the staging tile's phase
+        for (int unit = unit0; unit < n_units; unit += unit_step, ++done) {
+            const int sp = BRES ? 0 : unit - (unit / p.splits) * p.splits;
+            const int kb0 = sp * p.kb_per_split, kb1 = min(p.num_kb, kb0 + p.kb_per_split);
+            // ---- main loop: one wgmma group per stage, at most one group in flight behind the newest
+            float acc[BN / 2];
+#pragma unroll
+            for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+            int prev = -1;
+            for (int kb = kb0; kb < kb1; ++kb, ++it) {
+                const int stage = it % STAGES;
+                tc::mbar_wait(&full[stage], (it / STAGES) & 1);
+                const uint32_t a_base = tc::smem_u32(sA + stage * A_TILE_BYTES) + wg * (64 * 128);
+                const uint32_t b_base = tc::smem_u32(sB + (BRES ? kb : stage) * B_TILE_BYTES);
+                tc::wgmma_fence();
+#pragma unroll
+                for (int k = 0; k < BK / 16; ++k)
+                    tc::wgmma_ss<BN>(acc, tc::make_desc_sw128(a_base + k * 32), tc::make_desc_sw128(b_base + k * 32), 1u);
+                tc::wgmma_commit();
+                tc::wgmma_wait<1>();                 // the group of the previous stage has completed: release that stage
+                tc::reg_fence<BN / 2>(acc);
+                if (prev >= 0) tc::mbar_arrive(&empty[prev]);
+                prev = stage;
+            }
+            tc::wgmma_wait<0>();
+            tc::reg_fence<BN / 2>(acc);
+            if (prev >= 0) tc::mbar_arrive(&empty[prev]);
+
+            // ---- accumulators -> fp32 staging tile, once the epilogue warps are done with the previous unit's
+            tc::mbar_wait(stg_empty, (done & 1) ^ 1);
+#pragma unroll
+            for (int i = 0; i < BN / 8; ++i) {
+                const int c = 8 * i + frag_col;
+                *reinterpret_cast<float2*>(stg + frag_row * PITCH + c) = make_float2(acc[4 * i], acc[4 * i + 1]);
+                *reinterpret_cast<float2*>(stg + (frag_row + 8) * PITCH + c) = make_float2(acc[4 * i + 2], acc[4 * i + 3]);
+            }
+            tc::mbar_arrive(stg_full);
+        }
+        return;
+    }
+
+    // ---------------------------------------------------------------- epilogue (threads 288-511)
+    constexpr int RUNS = BM * (BN / 32);         // 32-column runs of one row each: run r = row r % BM, columns 32 (r / BM) ...
     // 64 bytes (one 32-column run of fp16 side input) as four 128-bit loads
     auto ld64 = [](const __half* src, uint4* q4) {
         const uint4* s4 = reinterpret_cast<const uint4*>(src);
 #pragma unroll
         for (int j = 0; j < 4; ++j) q4[j] = s4[j];
     };
-    if constexpr (BRES) tc::mbar_wait(b_full, 0);
-    int it = 0;
-    for (int unit = unit0; unit < n_units; unit += unit_step) {
+    int done = 0;
+    for (int unit = unit0; unit < n_units; unit += unit_step, ++done) {
         const int tile = BRES ? unit * p.tiles_n + nb_fixed : unit / p.splits, sp = BRES ? 0 : unit - (unit / p.splits) * p.splits;
-        const int kb0 = sp * p.kb_per_split, kb1 = min(p.num_kb, kb0 + p.kb_per_split);
-        // ---- main loop: one wgmma group per stage, at most one group in flight behind the newest
-        float acc[BN / 2];
-#pragma unroll
-        for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
-        int prev = -1;
-        for (int kb = kb0; kb < kb1; ++kb, ++it) {
-            const int stage = it % STAGES;
-            tc::mbar_wait(&full[stage], (it / STAGES) & 1);
-            const uint32_t a_base = tc::smem_u32(sA + stage * A_TILE_BYTES) + wg * (64 * 128);
-            const uint32_t b_base = tc::smem_u32(sB + (BRES ? kb : stage) * B_TILE_BYTES);
-            tc::wgmma_fence();
-#pragma unroll
-            for (int k = 0; k < BK / 16; ++k)
-                tc::wgmma_ss<BN>(acc, tc::make_desc_sw128(a_base + k * 32), tc::make_desc_sw128(b_base + k * 32), 1u);
-            tc::wgmma_commit();
-            tc::wgmma_wait<1>();                 // the group of the previous stage has completed: release that stage
-            tc::reg_fence<BN / 2>(acc);
-            if (prev >= 0) tc::mbar_arrive(&empty[prev]);
-            prev = stage;
-        }
-        tc::wgmma_wait<0>();
-        tc::reg_fence<BN / 2>(acc);
-        if (prev >= 0) tc::mbar_arrive(&empty[prev]);
-
-        // ---- accumulators -> fp32 staging tile (the previous unit's epilogue must be done reading it)
-        named_bar_sync(1, 256);
-#pragma unroll
-        for (int i = 0; i < BN / 8; ++i) {
-            const int c = 8 * i + frag_col;
-            *reinterpret_cast<float2*>(stg + frag_row * PITCH + c) = make_float2(acc[4 * i], acc[4 * i + 1]);
-            *reinterpret_cast<float2*>(stg + (frag_row + 8) * PITCH + c) = make_float2(acc[4 * i + 2], acc[4 * i + 3]);
-        }
-        named_bar_sync(1, 256);
-
-        // ---- epilogue: thread (row, half_id) takes the 32-column runs half_id, half_id + 2, ... of its row
         const int z = tile / tiles_mn, mn = tile - z * tiles_mn;
         const int m_blk = mn / p.tiles_n, n_blk = mn - m_blk * p.tiles_n;
         const int b1 = z % p.batch1, b2 = z / p.batch1;
-        bool row_ok;
-        long out_off, res_off;
-        int img = 0;
-        if (!p.conv) {
-            const int m = m_blk * BM + row;
-            row_ok = m < p.M;
-            out_off = static_cast<long>(b2) * p.so2 + static_cast<long>(b1) * p.so1 + static_cast<long>(m) * p.ldo;
-            res_off = static_cast<long>(b2) * p.sr2 + static_cast<long>(b1) * p.sr1 + static_cast<long>(m) * p.ldr;
-        } else {
-            const int tx = m_blk % p.tiles_x, ty = (m_blk / p.tiles_x) % p.tiles_y, tb = m_blk / (p.tiles_x * p.tiles_y);
-            const int xi = row % p.bw, yi = (row / p.bw) % p.bh, bi = row / (p.bw * p.bh);
-            const int x = tx * p.bw + xi, y = ty * p.bh + yi;
-            img = tb * p.bb + bi;
-            row_ok = (x < p.Wo) && (y < p.Ho) && (img < p.Bn);
-            const long pix = (static_cast<long>(img) * p.HoF + (y * p.osy + p.ooy)) * p.WoF + (x * p.osx + p.oox);
-            out_off = pix * p.ldo;
-            res_off = pix * p.ldr;
+        int tx = 0, ty = 0, tb = 0;
+        if (p.conv) {
+            tx = m_blk % p.tiles_x;
+            ty = (m_blk / p.tiles_x) % p.tiles_y;
+            tb = m_blk / (p.tiles_x * p.tiles_y);
         }
-        const int m_glob = m_blk * BM + row;
-        const float bias_row = (p.bias_mode == 2 && row_ok) ? __half2float(p.bias[m_glob]) : 0.f;
+        tc::mbar_wait(stg_full, done & 1);
+        // thread t takes the runs t, t + EPI_THREADS, ...: a warp reads 32 consecutive rows of one column range
 #pragma unroll 1
-        for (int c0 = half_id * 32; c0 < BN; c0 += 64) {
-            const int n0 = n_blk * BN + c0;
-            if (!row_ok || n0 >= p.N) continue;
+        for (int r = threadIdx.x - EPI_THREAD0; r < RUNS; r += EPI_THREADS) {
+            const int row = r % BM, c0 = (r / BM) * 32;
             float f[32];
 #pragma unroll
             for (int i = 0; i < 8; ++i) {
                 const float4 t = *reinterpret_cast<const float4*>(stg + row * PITCH + c0 + 4 * i);
                 f[4 * i] = t.x; f[4 * i + 1] = t.y; f[4 * i + 2] = t.z; f[4 * i + 3] = t.w;
             }
+            if (r + EPI_THREADS >= RUNS) tc::mbar_arrive(stg_empty);   // this thread's last staging read of the unit
+            bool row_ok;
+            long out_off, res_off;
+            int img = 0;
+            if (!p.conv) {
+                const int m = m_blk * BM + row;
+                row_ok = m < p.M;
+                out_off = static_cast<long>(b2) * p.so2 + static_cast<long>(b1) * p.so1 + static_cast<long>(m) * p.ldo;
+                res_off = static_cast<long>(b2) * p.sr2 + static_cast<long>(b1) * p.sr1 + static_cast<long>(m) * p.ldr;
+            } else {
+                const int xi = row % p.bw, yi = (row / p.bw) % p.bh, bi = row / (p.bw * p.bh);
+                const int x = tx * p.bw + xi, y = ty * p.bh + yi;
+                img = tb * p.bb + bi;
+                row_ok = (x < p.Wo) && (y < p.Ho) && (img < p.Bn);
+                const long pix = (static_cast<long>(img) * p.HoF + (y * p.osy + p.ooy)) * p.WoF + (x * p.osx + p.oox);
+                out_off = pix * p.ldo;
+                res_off = pix * p.ldr;
+            }
+            const int n0 = n_blk * BN + c0;
+            if (!row_ok || n0 >= p.N) continue;
+            const float bias_row = p.bias_mode == 2 ? __half2float(p.bias[m_blk * BM + row]) : 0.f;
             if (p.splits > 1) {   // raw partial sums; ws rows are dense with pitch N in output-row order
                 float* wp = p.ws + sp * p.ws_split_stride + (out_off / p.ldo) * p.N + n0;
                 if (n0 + 32 <= p.N && (p.N & 3) == 0) {
