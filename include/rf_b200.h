@@ -132,6 +132,15 @@ int rf_mel_to_wave_profiled(rf_plan* plan, const float* d_mel, const void* d_ini
                             int T, int n_iter, float momentum, float* d_wave, void* d_workspace,
                             size_t workspace_bytes, void* stream, float* ms_out, int* launches_out);
 
+/* Periodic inverse mel + Griffin-Lim for seamless loops: the waveform is one period of a signal of length L = hop * T,
+ * frame t centred at sample t * hop, every sample index taken modulo L (no reflect padding); the overlap-add is
+ * normalised by the periodic window-square sum, which has no edge terms.  Same n_fft, window, iterations, momentum,
+ * initial angles and inverse mel as rf_mel_to_wave; the frame transforms are the generic engine's mixed-radix FFT.
+ *   d_mel f32[B][n_mels][T] -> d_wave f32[B][hop * T].  Requires a pruned plan with hop <= win_length. */
+size_t rf_mel_to_wave_periodic_workspace_bytes(const rf_plan* plan, int B, int T);
+int rf_mel_to_wave_periodic(rf_plan* plan, const float* d_mel, const void* d_init_angles, int B, int T, int n_iter,
+                            float momentum, float* d_wave, void* d_workspace, size_t workspace_bytes, void* stream);
+
 /* ---- path (a), forward: waveform -> mel amplitudes ---------------------------------
  * replaces SpectrogramConverter.mel_amplitudes_from_waveform
  * (riffusion/spectrogram_converter.py:165-185): Spectrogram(power=None) -> abs -> MelScale.
@@ -226,7 +235,10 @@ typedef struct rf_conv_desc {
                                      (diffusers VAE Downsample2D: F.pad(x, (0,1,0,1)) then conv padding=0)
                                   2: nearest-2x upsample fused in (diffusers Upsample2D: F.interpolate(scale 2, nearest) then
                                      conv 3x3 pad 1): ksize = 2, w = the four sub-pixel phase kernels [4][Cout][2][2][C1]
-                                     (3x3 taps that land on the same input pixel pre-summed), out is [B][2H][2W][Cout] */
+                                     (3x3 taps that land on the same input pixel pre-summed), out is [B][2H][2W][Cout]
+                                  3: no padding: H, W include a one-pixel border already written into x1 (seamless loops:
+                                     rf_pad_wrap_w_f16); one input, 3x3, stride 1 or 2, out [B][(H-3)/stride+1][(W-3)/stride+1]
+                                  4: pad_mode 2 on such an input: out is [B][2(H-2)][2(W-2)][Cout] */
     void* workspace;           /* optional split-K scratch, as in rf_gemm_desc */
     int64_t workspace_bytes;
 } rf_conv_desc;
@@ -283,6 +295,15 @@ int rf_conv_in_f16(const void* x_nchw, const void* w, const void* bias, int B, i
 /* conv_out: Conv2d(Cin -> Cout<=8, 3x3, pad 1) reading NHWC, writing NCHW fp16; w packed [Cout][3][3][Cin] */
 int rf_conv_out_f16(const void* x_nhwc, const void* w_packed, const void* bias, int B, int H, int W, int Cin,
                     int Cout, void* y_nchw, void* stream);
+/* Seamless loops: conv_in / conv_out with circular padding along W and zero padding along H
+ * (F.pad(x, (1, 1, 0, 0), mode="circular") then Conv2d(padding=(1, 0))); same arguments and kernels */
+int rf_conv_in_wrap_f16(const void* x_nchw, const void* w, const void* bias, int B, int Cin, int H, int W, int Cout,
+                        void* y_nhwc, void* stream);
+int rf_conv_out_wrap_f16(const void* x_nhwc, const void* w_packed, const void* bias, int B, int H, int W, int Cin,
+                         int Cout, void* y_nchw, void* stream);
+/* One-pixel border for rf_conv2d_f16 pad_mode 3 / 4: x [B][H][W][C] -> y [B][H+2][W+2][C], rows 0 and H+1 zero, column 0
+ * = column W-1 of x, column W+1 = column 0 of x.  C % 8 == 0, pointers 16-byte aligned. */
+int rf_pad_wrap_w_f16(const void* x, int B, int H, int W, int C, void* y, void* stream);
 /* diffusers Timesteps(dim, flip_sin_to_cos=True, downscale_freq_shift=0): t fp32 [B] -> fp16 [B][dim] */
 int rf_timestep_embedding_f16(const float* d_t, int B, int dim, void* out, void* stream);
 int rf_silu_f16(const void* x, long n, void* y, void* stream);

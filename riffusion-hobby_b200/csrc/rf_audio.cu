@@ -3,6 +3,7 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
+#include <climits>
 #include <cmath>
 #include <cstring>
 #include <mutex>
@@ -11,6 +12,7 @@
 
 #include "rf_common.h"
 #include "rf_generic.cuh"
+#include "rf_periodic.cuh"
 #include "rf_gl_phases.cuh"
 #include "rf_plan.h"
 #include "rf_tc.cuh"
@@ -137,7 +139,7 @@ static int rf_plan_upload(rf_plan* p) {
         RF_CUDA_TRY(upload(p, &p->d5e_wg_inv, h.t5e.wg_inv.data(), h.t5e.wg_inv.size() / 4));
         RF_CUDA_TRY(upload(p, &p->d5e_ab_inv, h.t5e.ab_inv.data(), h.t5e.ab_inv.size() / 4));
     }
-    if (h.generic) {
+    if (h.mixed_radix) {
         RF_CUDA_TRY(upload(p, &p->d_window, h.window.data(), h.window.size()));
         RF_CUDA_TRY(upload(p, &p->d_roots2, h.roots2.data(), h.roots2.size() / 2));
         RF_CUDA_TRY(upload(p, &p->d_rootsN, h.rootsN.data(), h.rootsN.size() / 2));
@@ -1120,6 +1122,83 @@ extern "C" int rf_mel_to_wave_profiled(rf_plan* p, const float* d_mel, const voi
     }
     if (rc) return rc;
     if (e != cudaSuccess) return rf_fail(RF_ERR_CUDA, std::string("cudaStreamSynchronize: ") + cudaGetErrorString(e));
+    return RF_OK;
+}
+
+// ---- periodic Griffin-Lim (seamless loops): frames [B][T][W] of the generic engine, waveform [B][T * hop] -------------
+struct per_ws {
+    float* S;
+    rf_c32* R[2];
+    float* frames;
+    size_t total;
+};
+
+static per_ws per_layout(const rf_plan* p, int B, int T, void* base) {
+    per_ws w;
+    const size_t bt = static_cast<size_t>(B) * T * p->h.n_live;
+    unsigned char* b = static_cast<unsigned char*>(base);
+    size_t off = 0;
+    w.S = reinterpret_cast<float*>(b + off);
+    off += align256(bt * 4);
+    w.R[0] = reinterpret_cast<rf_c32*>(b + off);
+    off += align256(bt * 8);
+    w.R[1] = reinterpret_cast<rf_c32*>(b + off);
+    off += align256(bt * 8);
+    w.frames = reinterpret_cast<float*>(b + off);
+    off += align256(static_cast<size_t>(B) * T * p->h.W * 4);
+    w.total = off;
+    return w;
+}
+
+extern "C" size_t rf_mel_to_wave_periodic_workspace_bytes(const rf_plan* p, int B, int T) {
+    if (!p || B <= 0 || T <= 0) return 0;
+    return per_layout(p, B, T, nullptr).total;
+}
+
+extern "C" int rf_mel_to_wave_periodic(rf_plan* p, const float* d_mel, const void* d_init_angles, int B, int T, int n_iter,
+                                       float momentum, float* d_wave, void* d_ws, size_t ws_bytes, void* stream) {
+    const char* who = "rf_mel_to_wave_periodic";
+    if (!p || !d_mel || !d_wave || !d_ws || B <= 0 || T <= 0 || n_iter < 0)
+        return rf_fail(RF_ERR_INVALID, std::string(who) + ": bad argument");
+    if (!(momentum >= 0.f && momentum < 1.f))
+        return rf_fail(RF_ERR_INVALID, "momentum must be in range [0, 1). Found: " + std::to_string(momentum));
+    const rf_plan_host& h = p->h;
+    if (!h.mixed_radix)
+        return rf_fail(RF_ERR_UNSUPPORTED, std::string(who) + ": n_fft / 2 must be 2^a 3^b 5^c 7^d <= 14000");
+    if (h.H > h.W)
+        return rf_fail(RF_ERR_INVALID, std::string(who) + ": hop_length > win_length leaves samples no frame covers");
+    if (static_cast<long>(T) * h.H > INT32_MAX / 2) return rf_fail(RF_ERR_INVALID, std::string(who) + ": too many frames");
+    int rc = rf_plan_upload(p);
+    if (rc) return rc;
+    if ((rc = set_smem_attrs())) return rc;
+    if ((rc = gen_smem_attrs(p))) return rc;
+    static rf_dev_once once;
+    RF_CUDA_TRY(rf_set_smem_once(once, k_per_stft, 227 * 1024));
+    const per_ws w = per_layout(p, B, T, d_ws);
+    if (ws_bytes < w.total) return rf_fail(RF_ERR_INVALID, std::string(who) + ": workspace too small");
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if ((rc = launch_inverse_mel(p, d_mel, B, T, 0, w.S, st))) return rc;
+    gl_ws gw{};                     // gl_prepare_angles writes the initial angles to R[1]
+    gw.R[1] = w.R[1];
+    if ((rc = gl_prepare_angles(p, gw, d_init_angles, B, T, st))) return rc;
+    const rf_gen_tab g = make_gen_tab(p);
+    const size_t smem = gen_smem(p);
+    const int L = h.H * T;
+    const int c0 = h.N / 2 - (h.N - h.W) / 2;
+    // the recurrence and buffer rotation of gl_loop / gl_loop_generic (TA/functional/functional.py:300-340)
+    const float m = static_cast<float>(static_cast<double>(momentum) / (1.0 + static_cast<double>(momentum)));
+    const dim3 grid_f(T, B), grid_a((L + 255) / 256, B);
+    for (int it = 0; it <= n_iter; ++it) {
+        const rf_c32* cur = it == 0 ? w.R[1] : w.R[(it - 1) & 1];
+        const rf_c32* prev = (it >= 2 && m != 0.f) ? w.R[it & 1] : nullptr;
+        k_gen_istft<<<grid_f, 256, smem, st>>>(g, w.S, cur, prev, it == 0 ? 0 : 1, m, T, w.frames);
+        RF_CUDA_LAUNCH_CHECK("k_gen_istft");
+        k_per_ola<<<grid_a, 256, 0, st>>>(w.frames, p->d_win2, T, h.H, h.W, c0, L, d_wave);
+        RF_CUDA_LAUNCH_CHECK("k_per_ola");
+        if (it == n_iter) break;
+        k_per_stft<<<grid_f, 256, smem, st>>>(g, d_wave, L, T, w.R[it & 1]);
+        RF_CUDA_LAUNCH_CHECK("k_per_stft");
+    }
     return RF_OK;
 }
 

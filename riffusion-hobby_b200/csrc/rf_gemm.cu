@@ -734,10 +734,15 @@ extern "C" size_t rf_gemm_workspace_bytes(const rf_gemm_desc* d) {
 static int conv_impl(const rf_conv_desc* d, void* stream, size_t* query) {
     if (!d || !d->x1 || !d->w || !d->out || d->B <= 0 || d->H <= 0 || d->W <= 0 || d->C1 <= 0 || d->Cout <= 0)
         return rf_fail(RF_ERR_INVALID, "rf_conv2d_f16: bad argument");
-    const bool up2 = d->pad_mode == 2;      // nearest-2x upsample fused in: four 2x2 sub-pixel convolutions
+    if (d->pad_mode < 0 || d->pad_mode > 4) return rf_fail(RF_ERR_INVALID, "rf_conv2d_f16: pad_mode must be 0 to 4");
+    const bool up2 = d->pad_mode == 2 || d->pad_mode == 4;   // nearest-2x upsample fused in: four 2x2 sub-pixel convolutions
+    const int halo = d->pad_mode >= 3 ? 1 : 0;  // x1 carries its one-pixel border (rf_pad_wrap_w_f16): read it, pad nothing
     if (up2 && (d->ksize != 2 || d->stride != 1 || d->x2 || d->residual))
-        return rf_fail(RF_ERR_UNSUPPORTED, "rf_conv2d_f16: pad_mode 2 (fused upsample) takes ksize 2 phase weights, stride 1, "
-                                           "one input, no residual");
+        return rf_fail(RF_ERR_UNSUPPORTED, "rf_conv2d_f16: pad_mode 2 / 4 (fused upsample) takes ksize 2 phase weights, "
+                                           "stride 1, one input, no residual");
+    if (halo && (d->x2 || (!up2 && d->ksize != 3) || d->H < 3 || d->W < 3))
+        return rf_fail(RF_ERR_UNSUPPORTED, "rf_conv2d_f16: pad_mode 3 / 4 (input with a one-pixel border) takes a 3x3 or "
+                                           "fused-upsample convolution of one input of at least 3x3 pixels");
     if (!up2 && d->ksize != 1 && d->ksize != 3) return rf_fail(RF_ERR_UNSUPPORTED, "rf_conv2d_f16: kernel size must be 1 or 3");
     if (d->stride != 1 && d->stride != 2) return rf_fail(RF_ERR_UNSUPPORTED, "rf_conv2d_f16: stride must be 1 or 2");
     if ((d->C1 % BK) || (d->x2 && (d->C2 % BK)))
@@ -745,8 +750,9 @@ static int conv_impl(const rf_conv_desc* d, void* stream, size_t* query) {
                                            "convolution for the 4- and 3-channel layers)");
     const int pad = (d->ksize == 3 && d->pad_mode == 0) ? 1 : 0;
     const int extra = (d->ksize == 3 && d->pad_mode == 1) ? 1 : 0;   // one implicit zero row/column at the far edge
-    const int Ho = up2 ? d->H : (d->H + 2 * pad + extra - d->ksize) / d->stride + 1;   // up2: the tile grid is the input grid
-    const int Wo = up2 ? d->W : (d->W + 2 * pad + extra - d->ksize) / d->stride + 1;
+    // up2: the tile grid is the input grid (without its border); pad_mode 3 is a 3x3 convolution with padding 0
+    const int Ho = up2 ? d->H - 2 * halo : (d->H + 2 * pad + extra - d->ksize) / d->stride + 1;
+    const int Wo = up2 ? d->W - 2 * halo : (d->W + 2 * pad + extra - d->ksize) / d->stride + 1;
     // output pixels per tile.  bw is a power of two (it must divide 128): among those from min(8, bw_max) up to bw_max,
     // the largest power of two <= min(Wo, 128), take the one that pads Wo least, the larger one on a tie.  Powers of two
     // keep bw = Wo; 96-, 48- and 24-wide levels (768-pixel-wide clips) get exact 32-, 16- and 8-wide tiles instead of
@@ -828,7 +834,7 @@ static int conv_impl(const rf_conv_desc* d, void* stream, size_t* query) {
     p.osx = 2; p.osy = 2; p.HoF = 2 * Ho; p.WoF = 2 * Wo;
     for (int ph = 0; ph < 4; ++ph) {
         const int py = ph >> 1, px = ph & 1;
-        p.off_y = py - 1; p.off_x = px - 1;
+        p.off_y = py - 1 + halo; p.off_x = px - 1 + halo;
         p.ooy = py; p.oox = px;
         CUtensorMap mph;
         const long dims[4] = {Ktot, d->Cout, 1, 1};

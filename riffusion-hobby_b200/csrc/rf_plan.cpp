@@ -184,21 +184,26 @@ std::string rf_plan_build_host(const rf_plan_desc& d, const float* window, const
     p.generic = d.win_length != RF_W || d.n_fft != RF_N || d.hop_length > RF_W || (RF_W % d.hop_length) != 0;
     if (p.generic) {
         if (d.n_fft & 1) return "rf_plan_create: n_fft must be even (generic FFT engine packs two real samples per point)";
-        int n2 = d.n_fft / 2;
-        if (n2 > 14000)
+        if (d.n_fft / 2 > 14000)
             return "rf_plan_create: n_fft = " + std::to_string(d.n_fft) + " exceeds the generic engine's shared-memory frame "
                    "(n_fft <= 28000, i.e. sample rates up to 70 kHz with the default 400 ms padding)";
+    }
+    // the generic engine's radices, also those of the periodic (loop) Griffin-Lim on every plan: the prime-factor geometry's
+    // n_fft / 2 = 8820 = 4 * 3 * 3 * 5 * 7 * 7 always factors
+    {
+        int n2 = d.n_fft / 2;
         p.radices.clear();
         const int cand[5] = {4, 2, 3, 5, 7};
         for (int r : cand)
-            while (n2 % r == 0 && !(r == 2 && n2 % 4 == 0)) {
+            while (n2 > 0 && n2 % r == 0 && !(r == 2 && n2 % 4 == 0)) {
                 p.radices.push_back(r);
                 n2 /= r;
             }
-        if (n2 != 1)
+        if (p.generic && n2 != 1)
             return "rf_plan_create: n_fft/2 = " + std::to_string(d.n_fft / 2) + " has a prime factor > 7; the generic FFT engine "
                    "handles 2^a 3^b 5^c 7^d";
-        if (p.radices.size() > 16) return "rf_plan_create: too many FFT stages";
+        if (p.generic && p.radices.size() > 16) return "rf_plan_create: too many FFT stages";
+        p.mixed_radix = n2 == 1 && p.radices.size() <= 16 && (d.n_fft % 2) == 0 && d.n_fft / 2 <= 14000;
     }
     p.d = d;
     p.N = d.n_fft;
@@ -293,7 +298,7 @@ std::string rf_plan_build_host(const rf_plan_desc& d, const float* window, const
                   (idx2 << 15) | (static_cast<uint32_t>(k & 7) << 28);
     }
 
-    if (p.generic) {
+    if (p.mixed_radix) {
         const int N2 = p.N / 2;
         p.roots2.resize(static_cast<size_t>(N2) * 2);
         for (int n = 0; n < N2; ++n) {

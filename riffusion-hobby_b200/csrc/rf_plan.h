@@ -62,6 +62,7 @@ struct rf_plan_host {
     // generic engine (any other STFT geometry with n_fft = 2 * (2^a 3^b 5^c 7^d), e.g. 48 kHz: n_fft 19200, 22.05 kHz: 8820):
     // mixed-radix Stockham FFT of n_fft/2 complex points per frame in shared memory; bins in natural order
     bool generic = false;
+    bool mixed_radix = false;      // radices / roots2 / rootsN are built: the generic engine and the periodic Griffin-Lim
     std::vector<int> radices;      // product == n_fft / 2
     std::vector<float> roots2;     // [n_fft/2][2]    exp(-2 pi i n / (n_fft/2))
     std::vector<float> rootsN;     // [n_fft/2 + 1][2] exp(-2 pi i k / n_fft)

@@ -434,9 +434,44 @@ __global__ void k_upsample2x(const __half* __restrict__ x, int B, int H, int W, 
 }
 
 // ---------------------------------------------------------------- edge convolutions (tiny channel counts)
+// column index of a tap: as is (zero padding: the caller's bounds check drops it) or wrapped into [0, W) (xx >= -1,
+// xx <= W: taps reach one column past either edge)
+template <bool WRAP>
+__device__ __forceinline__ int rf_wrap_col(int xx, int W) {
+    if (!WRAP) return xx;
+    return xx < 0 ? xx + W : (xx >= W ? xx - W : xx);
+}
+
+// one-pixel border for the 3x3 convolutions of seamless loops: x [B][H][W][C] -> y [B][H+2][W+2][C] with zero rows on top
+// and bottom and wrapped columns left and right (torch: F.pad(F.pad(x, circular along W), zeros along H)).  16-byte
+// vectors (C % 8 == 0).
+__global__ void k_pad_wrap_w(const __half* __restrict__ x, int B, int H, int W, int C, __half* __restrict__ y) {
+    const int C8 = C / 8, Wp = W + 2, Hp = H + 2;
+    const size_t n = static_cast<size_t>(B) * Hp * Wp * C8;
+    const uint4* xs = reinterpret_cast<const uint4*>(x);
+    uint4* ys = reinterpret_cast<uint4*>(y);
+    for (size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < n;
+         i += static_cast<size_t>(gridDim.x) * blockDim.x) {
+        const int c = static_cast<int>(i % C8);
+        size_t p = i / C8;
+        const int xo = static_cast<int>(p % Wp);
+        p /= Wp;
+        const int yo = static_cast<int>(p % Hp);
+        const int b = static_cast<int>(p / Hp);
+        if (yo == 0 || yo == Hp - 1) {
+            ys[i] = make_uint4(0u, 0u, 0u, 0u);
+        } else {
+            const int xi = xo == 0 ? W - 1 : (xo == Wp - 1 ? 0 : xo - 1);
+            ys[i] = xs[((static_cast<size_t>(b) * H + yo - 1) * W + xi) * C8 + c];
+        }
+    }
+}
+
 // conv_in: NCHW fp16 (B, Cin<=8, H, W) -> NHWC fp16 (B, H, W, Cout), 3x3 pad 1. weights [Cout][Cin][3][3] fp16.
 // CTA = 64 consecutive pixels (8 per warp); the weights are staged once per CTA, transposed to [k][cout] so that
 // lanes (consecutive couts) read conflict-free and write coalesced NHWC rows.
+// WRAP (every edge kernel below): circular padding along W, zeros along H (seamless loops); the taps are the same.
+template <bool WRAP>
 __global__ void k_conv_in_generic(const __half* __restrict__ x, const __half* __restrict__ w, const __half* __restrict__ bias,
                           int B, int Cin, int H, int W, int Cout, __half* __restrict__ y) {
     extern __shared__ float wsm[];  // [Cin*9][Cout]
@@ -457,7 +492,7 @@ __global__ void k_conv_in_generic(const __half* __restrict__ x, const __half* __
 #pragma unroll 1
         for (int k = 0; k < K; ++k) {
             const int c = k / 9, t = k - c * 9;
-            const int yy = yq + t / 3 - 1, xx = xq + t % 3 - 1;
+            const int yy = yq + t / 3 - 1, xx = rf_wrap_col<WRAP>(xq + t % 3 - 1, W);
             in[k] = (yy >= 0 && yy < H && xx >= 0 && xx < W)
                         ? __half2float(x[((static_cast<size_t>(b) * Cin + c) * H + yy) * W + xx])
                         : 0.f;
@@ -472,6 +507,7 @@ __global__ void k_conv_in_generic(const __half* __restrict__ x, const __half* __
 
 // conv_out: NHWC fp16 (B, H, W, Cin) -> NCHW fp16/fp32 (B, Cout<=8, H, W), 3x3 pad 1. weights packed [Cout][3][3][Cin].
 // One warp per output pixel; lanes split the channels.
+template <bool WRAP>
 __global__ void k_conv_out_generic(const __half* __restrict__ x, const __half* __restrict__ w, const __half* __restrict__ bias,
                            int B, int H, int W, int Cin, int Cout, __half* __restrict__ y) {
     const size_t pix = static_cast<size_t>(blockIdx.x) * (blockDim.x >> 5) + (threadIdx.x >> 5);
@@ -482,7 +518,7 @@ __global__ void k_conv_out_generic(const __half* __restrict__ x, const __half* _
 #pragma unroll
     for (int o = 0; o < 8; ++o) acc[o] = 0.f;
     for (int t = 0; t < 9; ++t) {
-        const int yy = yq + t / 3 - 1, xx = xq + t % 3 - 1;
+        const int yy = yq + t / 3 - 1, xx = rf_wrap_col<WRAP>(xq + t % 3 - 1, W);
         if (yy < 0 || yy >= H || xx < 0 || xx >= W) continue;
         const __half* xp = x + ((static_cast<size_t>(b) * H + yy) * W + xx) * Cin;
         for (int c = lane; c < Cin; c += 32) {
@@ -501,7 +537,7 @@ __global__ void k_conv_out_generic(const __half* __restrict__ x, const __half* _
 // {2 lane + 64 i}, i < NCO2 (half2 stores: one 128-byte row segment per warp store), weights fp32 [k][Cout] in shared
 // memory (LDS.64, conflict-free), the 3 x 6 x Cin input patch of the group staged per warp and read by broadcast.
 // Persistent grid: every CTA stages the weights once and its warps stride over the pixel groups.  Needs W % 4 == 0.
-template <int NCO2>
+template <int NCO2, bool WRAP>
 __global__ void __launch_bounds__(256)
 k_conv_in_blk(const __half* __restrict__ x, const __half* __restrict__ w, const __half* __restrict__ bias, int B, int Cin,
               int H, int W, __half* __restrict__ y) {
@@ -527,7 +563,7 @@ k_conv_in_blk(const __half* __restrict__ x, const __half* __restrict__ w, const 
         __syncwarp();
         for (int e = lane; e < 18 * Cin; e += 32) {
             const int c = e / 18, r = e - c * 18, dy = r / 6, col = r - dy * 6;
-            const int yy = yq + dy - 1, xx = x0 + col - 1;
+            const int yy = yq + dy - 1, xx = rf_wrap_col<WRAP>(x0 + col - 1, W);
             patch[e] = (yy >= 0 && yy < H && xx >= 0 && xx < W)
                            ? __half2float(x[((static_cast<size_t>(b) * Cin + c) * H + yy) * W + xx])
                            : 0.f;
@@ -568,7 +604,7 @@ k_conv_in_blk(const __half* __restrict__ x, const __half* __restrict__ w, const 
 // channel pairs {2 lane + 64 s}, s < NSTEP (coalesced 128-byte loads), weights fp32 in shared memory as
 // [tap][s][2 halves of the cout quad][lane][4] (LDS.128, conflict-free).  The 6 input columns of a kernel row are
 // loaded once and shared by the 3 horizontal taps of the 4 pixels.  Persistent grid.  Needs W % 4 == 0.
-template <int NSTEP>
+template <int NSTEP, bool WRAP>
 __global__ void __launch_bounds__(256)
 k_conv_out_blk(const __half* __restrict__ x, const __half* __restrict__ w, const __half* __restrict__ bias, int B, int H,
                int W, int Cout, __half* __restrict__ y) {
@@ -599,7 +635,7 @@ k_conv_out_blk(const __half* __restrict__ x, const __half* __restrict__ w, const
             const __half* row = x + ((static_cast<size_t>(b) * H + yy) * W) * Cin + 2 * lane;
 #pragma unroll
             for (int col = 0; col < 6; ++col) {
-                const int xx = x0 + col - 1;
+                const int xx = rf_wrap_col<WRAP>(x0 + col - 1, W);
                 const bool ok = xx >= 0 && xx < W;
 #pragma unroll
                 for (int s_ = 0; s_ < NSTEP; ++s_)
@@ -1070,71 +1106,104 @@ extern "C" int rf_vae_image_to_u8(const void* x_nchw, int B, int H, int W, uint8
     return RF_OK;
 }
 
-template <int NCO2>
+template <int NCO2, bool WRAP>
 static int launch_conv_in_blk(const void* x, const void* w, const void* bias, int B, int Cin, int H, int W, void* y,
                               cudaStream_t st) {
     const size_t smem = (static_cast<size_t>(64 * NCO2) * Cin * 9 + 8 * 18 * 8) * sizeof(float);
     static rf_dev_once once;
-    RF_CUDA_TRY(rf_set_smem_once(once, k_conv_in_blk<NCO2>, 96 * 1024));
+    RF_CUDA_TRY(rf_set_smem_once(once, k_conv_in_blk<NCO2, WRAP>, 96 * 1024));
     const long ngroups = static_cast<long>(B) * H * (W / 4);
     const unsigned grid = static_cast<unsigned>(std::min<long>((ngroups + 7) / 8, 2L * rf_num_sms()));
-    k_conv_in_blk<NCO2><<<grid, 256, smem, st>>>(static_cast<const __half*>(x), static_cast<const __half*>(w),
+    k_conv_in_blk<NCO2, WRAP><<<grid, 256, smem, st>>>(static_cast<const __half*>(x), static_cast<const __half*>(w),
                                                  static_cast<const __half*>(bias), B, Cin, H, W, static_cast<__half*>(y));
     RF_CUDA_LAUNCH_CHECK("k_conv_in_blk");
     return RF_OK;
 }
 
-extern "C" int rf_conv_in_f16(const void* x_nchw, const void* w, const void* bias, int B, int Cin, int H, int W,
-                              int Cout, void* y_nhwc, void* stream) {
-    if (!x_nchw || !w || !y_nhwc || B <= 0 || Cin <= 0 || Cin > 8 || Cout <= 0) return rf_fail(RF_ERR_INVALID, "rf_conv_in_f16: bad argument");
+template <bool WRAP>
+static int conv_in_impl(const void* x_nchw, const void* w, const void* bias, int B, int Cin, int H, int W, int Cout,
+                        void* y_nhwc, void* stream) {
+    if (!x_nchw || !w || !y_nhwc || B <= 0 || Cin <= 0 || Cin > 8 || Cout <= 0 || H <= 0 || W <= 0)
+        return rf_fail(RF_ERR_INVALID, WRAP ? "rf_conv_in_wrap_f16: bad argument" : "rf_conv_in_f16: bad argument");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     if (W % 4 == 0 && (!bias || (reinterpret_cast<uintptr_t>(bias) & 3) == 0) &&
         (reinterpret_cast<uintptr_t>(y_nhwc) & 3) == 0) {
-        if (Cout == 512) return launch_conv_in_blk<8>(x_nchw, w, bias, B, Cin, H, W, y_nhwc, st);   // VAE decoder
-        if (Cout == 320) return launch_conv_in_blk<5>(x_nchw, w, bias, B, Cin, H, W, y_nhwc, st);
-        if (Cout == 128) return launch_conv_in_blk<2>(x_nchw, w, bias, B, Cin, H, W, y_nhwc, st);
-        if (Cout == 64) return launch_conv_in_blk<1>(x_nchw, w, bias, B, Cin, H, W, y_nhwc, st);
+        if (Cout == 512) return launch_conv_in_blk<8, WRAP>(x_nchw, w, bias, B, Cin, H, W, y_nhwc, st);   // VAE decoder
+        if (Cout == 320) return launch_conv_in_blk<5, WRAP>(x_nchw, w, bias, B, Cin, H, W, y_nhwc, st);
+        if (Cout == 128) return launch_conv_in_blk<2, WRAP>(x_nchw, w, bias, B, Cin, H, W, y_nhwc, st);
+        if (Cout == 64) return launch_conv_in_blk<1, WRAP>(x_nchw, w, bias, B, Cin, H, W, y_nhwc, st);
     }
     const size_t smem = static_cast<size_t>(Cout) * Cin * 9 * sizeof(float);
     if (smem > 96 * 1024) return rf_fail(RF_ERR_UNSUPPORTED, "rf_conv_in_f16: weights too large");
     static rf_dev_once once;
-    RF_CUDA_TRY(rf_set_smem_once(once, k_conv_in_generic, 96 * 1024));
+    RF_CUDA_TRY(rf_set_smem_once(once, k_conv_in_generic<WRAP>, 96 * 1024));
     const size_t npix = static_cast<size_t>(B) * H * W;
-    k_conv_in_generic<<<static_cast<unsigned>((npix + 63) / 64), 256, smem, st>>>(
+    k_conv_in_generic<WRAP><<<static_cast<unsigned>((npix + 63) / 64), 256, smem, st>>>(
         static_cast<const __half*>(x_nchw), static_cast<const __half*>(w), static_cast<const __half*>(bias), B, Cin, H, W,
         Cout, static_cast<__half*>(y_nhwc));
     RF_CUDA_LAUNCH_CHECK("k_conv_in");
     return RF_OK;
 }
 
-template <int NSTEP>
+extern "C" int rf_conv_in_f16(const void* x_nchw, const void* w, const void* bias, int B, int Cin, int H, int W,
+                              int Cout, void* y_nhwc, void* stream) {
+    return conv_in_impl<false>(x_nchw, w, bias, B, Cin, H, W, Cout, y_nhwc, stream);
+}
+extern "C" int rf_conv_in_wrap_f16(const void* x_nchw, const void* w, const void* bias, int B, int Cin, int H, int W,
+                                   int Cout, void* y_nhwc, void* stream) {
+    return conv_in_impl<true>(x_nchw, w, bias, B, Cin, H, W, Cout, y_nhwc, stream);
+}
+
+template <int NSTEP, bool WRAP>
 static int launch_conv_out_blk(const void* x, const void* w, const void* bias, int B, int H, int W, int Cout, void* y,
                                cudaStream_t st) {
     const size_t smem = static_cast<size_t>(9) * NSTEP * 256 * sizeof(float);
     static rf_dev_once once;
-    RF_CUDA_TRY(rf_set_smem_once(once, k_conv_out_blk<NSTEP>, 96 * 1024));
+    RF_CUDA_TRY(rf_set_smem_once(once, k_conv_out_blk<NSTEP, WRAP>, 96 * 1024));
     const long ngroups = static_cast<long>(B) * H * (W / 4);
     const unsigned grid = static_cast<unsigned>(std::min<long>((ngroups + 7) / 8, 2L * rf_num_sms()));
-    k_conv_out_blk<NSTEP><<<grid, 256, smem, st>>>(static_cast<const __half*>(x), static_cast<const __half*>(w),
+    k_conv_out_blk<NSTEP, WRAP><<<grid, 256, smem, st>>>(static_cast<const __half*>(x), static_cast<const __half*>(w),
                                                    static_cast<const __half*>(bias), B, H, W, Cout, static_cast<__half*>(y));
     RF_CUDA_LAUNCH_CHECK("k_conv_out_blk");
     return RF_OK;
 }
 
-extern "C" int rf_conv_out_f16(const void* x_nhwc, const void* w_packed, const void* bias, int B, int H, int W, int Cin,
-                               int Cout, void* y_nchw, void* stream) {
-    if (!x_nhwc || !w_packed || !y_nchw || B <= 0 || Cout <= 0 || Cout > 8) return rf_fail(RF_ERR_INVALID, "rf_conv_out_f16: bad argument");
+template <bool WRAP>
+static int conv_out_impl(const void* x_nhwc, const void* w_packed, const void* bias, int B, int H, int W, int Cin, int Cout,
+                         void* y_nchw, void* stream) {
+    if (!x_nhwc || !w_packed || !y_nchw || B <= 0 || Cout <= 0 || Cout > 8 || H <= 0 || W <= 0)
+        return rf_fail(RF_ERR_INVALID, WRAP ? "rf_conv_out_wrap_f16: bad argument" : "rf_conv_out_f16: bad argument");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     if (W % 4 == 0 && Cout <= 4 && (reinterpret_cast<uintptr_t>(y_nchw) & 7) == 0) {
-        if (Cin == 320) return launch_conv_out_blk<5>(x_nhwc, w_packed, bias, B, H, W, Cout, y_nchw, st);
-        if (Cin == 128) return launch_conv_out_blk<2>(x_nhwc, w_packed, bias, B, H, W, Cout, y_nchw, st);
-        if (Cin == 64) return launch_conv_out_blk<1>(x_nhwc, w_packed, bias, B, H, W, Cout, y_nchw, st);
+        if (Cin == 320) return launch_conv_out_blk<5, WRAP>(x_nhwc, w_packed, bias, B, H, W, Cout, y_nchw, st);
+        if (Cin == 128) return launch_conv_out_blk<2, WRAP>(x_nhwc, w_packed, bias, B, H, W, Cout, y_nchw, st);
+        if (Cin == 64) return launch_conv_out_blk<1, WRAP>(x_nhwc, w_packed, bias, B, H, W, Cout, y_nchw, st);
     }
     const size_t pix = static_cast<size_t>(B) * H * W;
-    k_conv_out_generic<<<static_cast<unsigned>((pix + 7) / 8), 256, 0, st>>>(
+    k_conv_out_generic<WRAP><<<static_cast<unsigned>((pix + 7) / 8), 256, 0, st>>>(
         static_cast<const __half*>(x_nhwc), static_cast<const __half*>(w_packed), static_cast<const __half*>(bias), B, H,
         W, Cin, Cout, static_cast<__half*>(y_nchw));
     RF_CUDA_LAUNCH_CHECK("k_conv_out");
+    return RF_OK;
+}
+
+extern "C" int rf_conv_out_f16(const void* x_nhwc, const void* w_packed, const void* bias, int B, int H, int W, int Cin,
+                               int Cout, void* y_nchw, void* stream) {
+    return conv_out_impl<false>(x_nhwc, w_packed, bias, B, H, W, Cin, Cout, y_nchw, stream);
+}
+extern "C" int rf_conv_out_wrap_f16(const void* x_nhwc, const void* w_packed, const void* bias, int B, int H, int W,
+                                    int Cin, int Cout, void* y_nchw, void* stream) {
+    return conv_out_impl<true>(x_nhwc, w_packed, bias, B, H, W, Cin, Cout, y_nchw, stream);
+}
+
+extern "C" int rf_pad_wrap_w_f16(const void* x, int B, int H, int W, int C, void* y, void* stream) {
+    if (!x || !y || B <= 0 || H <= 0 || W <= 0 || C <= 0 || (C % 8) || (reinterpret_cast<uintptr_t>(x) & 15) ||
+        (reinterpret_cast<uintptr_t>(y) & 15))
+        return rf_fail(RF_ERR_INVALID, "rf_pad_wrap_w_f16: bad argument (C must be a multiple of 8, pointers 16-byte aligned)");
+    const size_t n = static_cast<size_t>(B) * (H + 2) * (W + 2) * (C / 8);
+    k_pad_wrap_w<<<grid_for(n, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(static_cast<const __half*>(x), B, H, W, C,
+                                                                                  static_cast<__half*>(y));
+    RF_CUDA_LAUNCH_CHECK("k_pad_wrap_w");
     return RF_OK;
 }
 

@@ -91,6 +91,9 @@ SIGNATURES = {
                                  C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     "rf_mel_to_wave_profiled": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_float,
                                           C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "rf_mel_to_wave_periodic_workspace_bytes": (C.c_size_t, [C.c_void_p, C.c_int, C.c_int]),
+    "rf_mel_to_wave_periodic": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_float,
+                                          C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     "rf_stft_mel": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     "rf_stft": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     "rf_mel_scale": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
@@ -113,6 +116,11 @@ SIGNATURES = {
                                  C.c_void_p, C.c_void_p]),
     "rf_conv_out_f16": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                                   C.c_void_p, C.c_void_p]),
+    "rf_conv_in_wrap_f16": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
+                                      C.c_void_p, C.c_void_p]),
+    "rf_conv_out_wrap_f16": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
+                                       C.c_void_p, C.c_void_p]),
+    "rf_pad_wrap_w_f16": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     "rf_timestep_embedding_f16": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     "rf_silu_f16": (C.c_int, [C.c_void_p, C.c_long, C.c_void_p, C.c_void_p]),
     "rf_slerp_f16": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_long, C.c_void_p, C.c_float, C.c_void_p, C.c_void_p,

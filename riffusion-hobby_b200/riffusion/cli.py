@@ -10,7 +10,7 @@ the same names, flags and defaults (`COMMANDS`, what `build_parser()` builds by 
     python -m riffusion.cli sample-clips-batch --audio-dir songs --output-dir clips
     python -m riffusion.cli text-to-audio --prompt "jazz with piano" --audio out.wav [--image out.png]
         [--negative-prompt ...] [--seed 42] [--num-clips 1] [--num-inference-steps 30] [--guidance 7.0] [--width 512]
-        [--scheduler DPMSolverMultistepScheduler] [--use-20k] [--checkpoint DIR] [--device cuda]
+        [--scheduler DPMSolverMultistepScheduler] [--use-20k] [--loop] [--checkpoint DIR] [--device cuda]
     python -m riffusion.cli audio-to-audio --audio song.wav --output riffed.wav --prompt "jazz with piano"
         [--image-dir clips] [--negative-prompt ...] [--seed 42] [--denoising 0.55] [--num-inference-steps 25]
         [--guidance 7.0] [--scheduler DPMSolverMultistepScheduler] [--start-time-s 0] [--duration-s 20]
@@ -26,7 +26,8 @@ the same names, flags and defaults (`COMMANDS`, what `build_parser()` builds by 
 
 `--scheduler` takes DPMSolverMultistepScheduler, PNDMScheduler, DDIMScheduler or EulerAncestralDiscreteScheduler
 (audio-to-audio's --magic-mix refuses the last).  `text-to-audio` loads a local diffusers-layout checkpoint directory; with `--num-clips N` > 1 clip i (seed + i) is
-written to out_<seed + i>.wav / .png.  The image carries the spectrogram parameters in its EXIF block, so
+written to out_<seed + i>.wav / .png.  `--loop` renders seamless loops: a clip of exactly hop * width samples whose
+spectrogram tiles horizontally and whose audio plays on repeat without a click.  The image carries the spectrogram parameters in its EXIF block, so
 `image-to-audio` turns it back into the same audio.
 
 Each command is a keyword-only function (callable from Python exactly like the reference's); `argh`, which the reference
@@ -208,9 +209,10 @@ def sample_clips_batch(*, audio_dir: str, output_dir: str, num_clips_per_file: i
 
 def text_to_audio(*, prompt: str, audio: str, image: str = "", negative_prompt: str = "", seed: int = 42,
                   num_clips: int = 1, num_inference_steps: int = 30, guidance: float = 7.0, width: int = 512,
-                  scheduler: str = "DPMSolverMultistepScheduler", use_20k: bool = False,
+                  scheduler: str = "DPMSolverMultistepScheduler", use_20k: bool = False, loop: bool = False,
                   checkpoint: str = "riffusion/riffusion-model-v1", device: str = "cuda"):
-    """Generate audio from a text prompt (Stable Diffusion txt2img, then spectrogram image -> audio)."""
+    """Generate audio from a text prompt (Stable Diffusion txt2img, then spectrogram image -> audio); with --loop, a
+    seamless loop."""
     from riffusion.riffusion_pipeline import RiffusionPipeline
     from riffusion.util import audio_util
 
@@ -218,7 +220,7 @@ def text_to_audio(*, prompt: str, audio: str, image: str = "", negative_prompt: 
     pipe = RiffusionPipeline.load_checkpoint(checkpoint=checkpoint, device=device)
     out = pipe.text_to_audio(prompt, params=params, negative_prompt=negative_prompt or None, seed=seed,
                              num_clips=num_clips, num_inference_steps=num_inference_steps, guidance_scale=guidance,
-                             width=width, scheduler=scheduler)
+                             width=width, scheduler=scheduler, **(dict(loop=True) if loop else {}))
     images, waves = out["images"].cpu().numpy(), out["waveform"].cpu().numpy()
 
     def target(path: str, i: int) -> Path:

@@ -13,7 +13,8 @@ import torch
 
 
 class GraphedUNet:
-    def __init__(self, unet, latent_shape: T.Sequence[int], context: torch.Tensor):
+    def __init__(self, unet, latent_shape: T.Sequence[int], context: torch.Tensor, wrap_w: bool = False):
+        """`wrap_w`: capture the UNet with circular padding along W (seamless loops)."""
         dev = unet.device
         B2 = context.shape[0]
         self.unet = unet
@@ -25,12 +26,12 @@ class GraphedUNet:
         side.wait_stream(torch.cuda.current_stream(dev))
         with torch.cuda.stream(side):
             for _ in range(2):      # warm-up: fills the K/V cache, sets kernel attributes, primes the allocator
-                unet(self.x, self.t, encoder_hidden_states=self.ctx, ctx_cache=self.cache)
+                unet(self.x, self.t, encoder_hidden_states=self.ctx, ctx_cache=self.cache, wrap_w=wrap_w)
         torch.cuda.current_stream(dev).wait_stream(side)
         torch.cuda.synchronize(dev)
         self.graph = torch.cuda.CUDAGraph()
         with torch.cuda.graph(self.graph):
-            self.out = unet(self.x, self.t, encoder_hidden_states=self.ctx, ctx_cache=self.cache).sample
+            self.out = unet(self.x, self.t, encoder_hidden_states=self.ctx, ctx_cache=self.cache, wrap_w=wrap_w).sample
 
     def set_context(self, context: torch.Tensor) -> None:
         """Re-target the captured graph to another text context of the same shape: the graph reads the context only

@@ -527,18 +527,20 @@ class RiffusionPipeline:
         out["nsfw_content_detected"] = False
         return out
 
-    def _graphed_unet(self, latent_shape, context: torch.Tensor):
-        """The CUDA-graph CFG evaluation for this (latent shape, context shape), or None when graphs are off."""
+    def _graphed_unet(self, latent_shape, context: torch.Tensor, wrap_w: bool = False):
+        """The CUDA-graph CFG evaluation for this (latent shape, context shape, wrap_w), or None when graphs are off."""
         if not self.use_cuda_graph:
             return None
         from riffusion.graphed import GraphedUNet
 
-        # one captured graph per (latent shape, context shape); a new request only refreshes the cross-attention
-        # K / V^T that the graph reads (capture costs two eager evaluations + instantiation)
-        gkey = (tuple(latent_shape), tuple(context.shape))
+        # one captured graph per (latent shape, context shape, loop mode); a new request only refreshes the
+        # cross-attention K / V^T that the graph reads (capture costs two eager evaluations + instantiation).  Loop and
+        # non-loop evaluations run different convolutions, so they never share a graph.
+        gkey = (tuple(latent_shape), tuple(context.shape)) + (("wrap_w",) if wrap_w else ())
         graphed = self._graphs.get(gkey)
         if graphed is None:
-            graphed = self._graphs[gkey] = GraphedUNet(self.unet, latent_shape, context)
+            graphed = self._graphs[gkey] = (GraphedUNet(self.unet, latent_shape, context, wrap_w=True) if wrap_w else
+                                            GraphedUNet(self.unet, latent_shape, context))
         else:
             graphed.set_context(context)
         return graphed
@@ -550,7 +552,7 @@ class RiffusionPipeline:
                 scheduler: str = "DPMSolverMultistepScheduler", output_type: T.Optional[str] = "pil",
                 text_embeddings: T.Optional[torch.Tensor] = None, uncond_embeddings: T.Optional[torch.Tensor] = None,
                 latents: T.Optional[torch.Tensor] = None,
-                step_noise: T.Optional[torch.Tensor] = None) -> T.Dict[str, T.Any]:
+                step_noise: T.Optional[torch.Tensor] = None, loop: bool = False) -> T.Dict[str, T.Any]:
         """Text to spectrogram image: Stable Diffusion txt2img, the reference app's text-to-audio generation.
 
         Clip i starts from `torch.randn((1, 4, height/8, width/8))` drawn from a CUDA generator seeded with `seed + i`
@@ -560,8 +562,9 @@ class RiffusionPipeline:
         instance is used per call.  Euler ancestral also draws one fp16 tensor per step from each clip's generator,
         after its latents (`_step_noise`).  `width` and `height` must be multiples of 64 (diffusers accepts multiples of
         8).  `text_embeddings` / `uncond_embeddings` / `latents` / `step_noise` (steps, clips, 4, h, w) replace the text
-        encoder and the generator draws.  Returns dict(images, latents (1/0.18215-scaled), latents_unscaled,
-        n_unet_evals)."""
+        encoder and the generator draws.  `loop`: every 3x3 convolution of the UNet and of the VAE decoder pads circularly
+        along the width, so the image tiles horizontally (a seamless loop).  Returns dict(images, latents
+        (1/0.18215-scaled), latents_unscaled, n_unet_evals)."""
         if width <= 0 or height <= 0 or width % 64 or height % 64:
             raise ValueError(f"width and height must be positive multiples of 64, got {width}x{height}")
         if num_clips < 1:
@@ -581,6 +584,9 @@ class RiffusionPipeline:
         self._step_noise(sched, len(sched.timesteps), latents, step_noise, gens)
         if sched.init_noise_sigma != 1.0:
             latents = (latents * sched.init_noise_sigma).contiguous()
+        if loop:        # the default call stays exactly what it was
+            latents, n_evals = self._denoise(sched, sched.timesteps, latents, context, guidance_scale, wrap_w=True)
+            return self._finish(latents, n_evals, output_type, wrap_w=True)
         latents, n_evals = self._denoise(sched, sched.timesteps, latents, context, guidance_scale)
         return self._finish(latents, n_evals, output_type)
 
@@ -629,7 +635,8 @@ class RiffusionPipeline:
     def _denoise(self, sched, timesteps, latents: torch.Tensor, context: torch.Tensor, guidance_scale: float,
                  mask: T.Optional[torch.Tensor] = None, init: T.Optional[torch.Tensor] = None,
                  noise: T.Optional[torch.Tensor] = None,
-                 layout: T.Optional[T.Tuple[float, torch.Tensor, torch.Tensor, int]] = None) -> T.Tuple[torch.Tensor, int]:
+                 layout: T.Optional[T.Tuple[float, torch.Tensor, torch.Tensor, int]] = None,
+                 wrap_w: bool = False) -> T.Tuple[torch.Tensor, int]:
         """The CFG loop over `timesteps`: one UNet evaluation of [latents | latents] (a captured CUDA graph when enabled)
         and one fused guidance + scheduler step each.  With a `mask`, every step is followed by the inpainting blend of
         interpolate_img2img (:420-425): `init` noised with `noise` at that step's timestep where the mask is 1, the
@@ -638,10 +645,13 @@ class RiffusionPipeline:
         noise32, t) (`tc_ops.magic_mix`) and the scheduler still steps the latents.  The UNet input passes through
         `sched.scale_model_input` (the identity, without a launch, for every scheduler but Euler ancestral).  The UNet,
         the graph and the scheduler receive the scheduler's own timestep values: ints, or floats for Euler ancestral.
-        Returns (latents, evaluations)."""
+        `wrap_w`: the UNet pads circularly along W (seamless loops).  Returns (latents, evaluations)."""
         do_cfg = guidance_scale > 1.0
         ctx_cache: T.Dict[str, T.Any] = {}
-        graphed = self._graphed_unet(latents.shape, context) if do_cfg else None
+        graphed = None
+        if do_cfg:
+            graphed = self._graphed_unet(latents.shape, context, True) if wrap_w else self._graphed_unet(latents.shape, context)
+        loop_kw = dict(wrap_w=True) if wrap_w else {}
         if mask is not None:
             mask = mask.to(device=latents.device, dtype=latents.dtype).expand_as(latents).contiguous()
         n_evals = 0
@@ -656,7 +666,7 @@ class RiffusionPipeline:
                 eps_pair = graphed(unet_in, t_val)
             else:
                 model_in = torch.cat([unet_in] * 2) if do_cfg else unet_in
-                eps_pair = self.unet(model_in, t_val, encoder_hidden_states=context, ctx_cache=ctx_cache).sample
+                eps_pair = self.unet(model_in, t_val, encoder_hidden_states=context, ctx_cache=ctx_cache, **loop_kw).sample
             n_evals += 1
             if not do_cfg:
                 eps_pair = torch.cat([eps_pair, eps_pair])
@@ -665,23 +675,28 @@ class RiffusionPipeline:
                 latents = sched.add_noise(init, noise, t_val, mask=mask, blend_with=latents)
         return latents, n_evals
 
-    def _finish(self, latents: torch.Tensor, n_evals: int, output_type: T.Optional[str]) -> T.Dict[str, T.Any]:
+    def _finish(self, latents: torch.Tensor, n_evals: int, output_type: T.Optional[str],
+                wrap_w: bool = False) -> T.Dict[str, T.Any]:
         """dict(latents (1/0.18215-scaled), latents_unscaled, n_unet_evals, images): PIL images, a float16 (B, H, W, 3)
-        array in [0, 1] for any other output_type, or None for "latent" and without a VAE."""
+        array in [0, 1] for any other output_type, or None for "latent" and without a VAE.  `wrap_w`: the decoder pads
+        circularly along W."""
         scaled = (1.0 / VAE_SCALE) * latents
         out: T.Dict[str, T.Any] = dict(latents=scaled, latents_unscaled=latents, n_unet_evals=n_evals)
         if output_type == "latent" or self.vae is None:
             out["images"] = None
         elif output_type == "pil":
-            out["images"] = [Image.fromarray(im) for im in self._decode_u8(scaled).cpu().numpy()]
+            u8 = self._decode_u8(scaled, True) if wrap_w else self._decode_u8(scaled)
+            out["images"] = [Image.fromarray(im) for im in u8.cpu().numpy()]
         else:
-            image = self.vae.decode(scaled).sample
+            image = (self.vae.decode(scaled, wrap_w=True) if wrap_w else self.vae.decode(scaled)).sample
             out["images"] = (image / 2 + 0.5).clamp(0, 1).cpu().permute(0, 2, 3, 1).numpy()
         return out
 
-    def _decode_u8(self, scaled_latents: torch.Tensor) -> torch.Tensor:
+    def _decode_u8(self, scaled_latents: torch.Tensor, wrap_w: bool = False) -> torch.Tensor:
         """VAE decode -> (B, H, W, 3) uint8 images: `(image / 2 + 0.5).clamp(0, 1)` -> numpy_to_pil (:430-434) in the fp16
-        arithmetic of the reference's CUDA path, on the device."""
+        arithmetic of the reference's CUDA path, on the device.  `wrap_w`: the decoder pads circularly along W."""
+        if wrap_w:
+            return ops.vae_image_to_u8(self.vae.decode(scaled_latents, wrap_w=True).sample)
         return ops.vae_image_to_u8(self.vae.decode(scaled_latents).sample)
 
     # ------------------------------------------------------------------------------ image -> image
@@ -825,13 +840,17 @@ class RiffusionPipeline:
                       text_embeddings: T.Optional[torch.Tensor] = None, uncond_embeddings: T.Optional[torch.Tensor] = None,
                       latents: T.Optional[torch.Tensor] = None, converter=None,
                       init_angles: T.Optional[torch.Tensor] = None,
-                      step_noise: T.Optional[torch.Tensor] = None) -> T.Dict[str, torch.Tensor]:
+                      step_noise: T.Optional[torch.Tensor] = None, loop: bool = False) -> T.Dict[str, torch.Tensor]:
         """Text to audio on the device: `txt2img` with height = params.num_frequencies, then VAE decode -> uint8 image ->
         mel amplitudes (`audio_from_spectrogram_image` semantics: R plane for mono, G and B for stereo, max_value 30e6)
         -> inverse mel + Griffin-Lim.  `params` defaults to mono 0-10 kHz; `scheduler`, `latents` and `step_noise` are
         txt2img's.  Returns device tensors: images (B, H, W, 3)
         uint8, waveform (B, channels, hop * (W - 1)) fp32 before peak normalisation, latents, latents_unscaled,
-        n_unet_evals."""
+        n_unet_evals.
+
+        `loop` renders a seamless loop: txt2img's `loop` (circular width padding in the UNet and the VAE decoder), then
+        the periodic Griffin-Lim (`waveform_from_mel_amplitudes(periodic=True)`), whose waveform of exactly hop * W
+        samples per channel plays on repeat without a seam."""
         params = DEFAULT_PARAMS if params is None else params
         if height is not None and height != params.num_frequencies:
             raise ValueError(f"height {height} differs from params.num_frequencies {params.num_frequencies}")
@@ -840,9 +859,13 @@ class RiffusionPipeline:
                            num_inference_steps=num_inference_steps, guidance_scale=guidance_scale, width=width,
                            height=params.num_frequencies, scheduler=scheduler, output_type="latent",
                            text_embeddings=text_embeddings, uncond_embeddings=uncond_embeddings, latents=latents,
-                           step_noise=step_noise)
-        u8 = self._decode_u8(out["latents"])
-        wave = self._u8_to_waveform(u8, converter, params.stereo, init_angles)
+                           step_noise=step_noise, **(dict(loop=True) if loop else {}))
+        if loop:
+            u8 = self._decode_u8(out["latents"], True)
+            wave = self._u8_to_waveform(u8, converter, params.stereo, init_angles, periodic=True)
+        else:
+            u8 = self._decode_u8(out["latents"])
+            wave = self._u8_to_waveform(u8, converter, params.stereo, init_angles)
         return dict(images=u8, waveform=wave, latents=out["latents"], latents_unscaled=out["latents_unscaled"],
                     n_unet_evals=out["n_unet_evals"])
 
@@ -925,8 +948,10 @@ class RiffusionPipeline:
         return converter
 
     @staticmethod
-    def _u8_to_waveform(u8: torch.Tensor, converter, stereo: bool, init_angles: T.Optional[torch.Tensor]) -> torch.Tensor:
-        """uint8 images (B, H, W, 3) -> mel amplitudes (B, channels, H, W) -> waveform (B, channels, L)."""
+    def _u8_to_waveform(u8: torch.Tensor, converter, stereo: bool, init_angles: T.Optional[torch.Tensor],
+                        periodic: bool = False) -> torch.Tensor:
+        """uint8 images (B, H, W, 3) -> mel amplitudes (B, channels, H, W) -> waveform (B, channels, L); `periodic`: the
+        loop Griffin-Lim, L = hop * W."""
         from riffusion import _native
 
         B, H, W, _ = _native.operand(u8, "u8", torch.uint8, shape=(_native.ANY, _native.ANY, _native.ANY, 3)).shape
@@ -935,6 +960,8 @@ class RiffusionPipeline:
         for i in range(B):
             _native.call("rf_image_to_mel", u8.device, u8[i].data_ptr(), H, W, int(stereo), float(p.power_for_image),
                          30e6, mel[i].data_ptr())
+        if periodic:
+            return converter.waveform_from_mel_amplitudes(mel, init_angles, periodic=True)
         return converter.waveform_from_mel_amplitudes(mel, init_angles)
 
     # ------------------------------------------------------------------------------ audio -> audio

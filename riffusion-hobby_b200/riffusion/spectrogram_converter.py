@@ -270,11 +270,15 @@ class SpectrogramConverter:
         return mel.reshape(tuple(lead) + mel.shape[-2:])
 
     def waveform_from_mel_amplitudes(
-        self, amplitudes_mel: torch.Tensor, init_angles: T.Optional[torch.Tensor] = None
+        self, amplitudes_mel: torch.Tensor, init_angles: T.Optional[torch.Tensor] = None, periodic: bool = False
     ) -> torch.Tensor:
         """(batch, n_mels, frames) -> (batch, hop*(frames-1)): inverse mel + Griffin-Lim, fused
         (spectrogram_converter.py:187-204).  `init_angles` (batch, n_freq, frames) complex64
-        overrides the random phase initialisation (used by the parity tests)."""
+        overrides the random phase initialisation (used by the parity tests).
+
+        `periodic` (seamless loops) -> (batch, hop*frames): the waveform is one period of a looping signal; frame t is
+        centred at sample t*hop and every sample index wraps around, so the end runs into the start without a seam
+        (include/rf_b200.h: rf_mel_to_wave_periodic)."""
         m, lead = _flatten(_native.require_cuda(amplitudes_mel, "amplitudes_mel", torch.float32), 2)
         plan = get_plan(self.p, full_band=False, device=m.device)
         B, n_mels, Tn = m.shape
@@ -284,6 +288,13 @@ class SpectrogramConverter:
         if init_angles is None:
             init_angles = torch.rand((B, F, Tn), dtype=torch.complex64, device=m.device)
         ang = _native.require_cuda(init_angles, "init_angles", torch.complex64).reshape(B, F, Tn)
+        if periodic:
+            wave = torch.empty((B, self.p.hop_length * Tn), dtype=torch.float32, device=m.device)
+            nbytes = _native.lib().rf_mel_to_wave_periodic_workspace_bytes(plan.handle, B, Tn)
+            ws = torch.empty(nbytes, dtype=torch.uint8, device=m.device)
+            _native.call("rf_mel_to_wave_periodic", m.device, plan.handle, m.data_ptr(), ang.data_ptr(), B, Tn,
+                         self.p.num_griffin_lim_iters, GriffinLim.momentum, wave.data_ptr(), ws.data_ptr(), nbytes)
+            return wave.reshape(tuple(lead) + wave.shape[-1:])
         wave = torch.empty((B, self.p.hop_length * (Tn - 1)), dtype=torch.float32, device=m.device)
         nbytes = _native.lib().rf_griffinlim_workspace_bytes(plan.handle, B, Tn)
         ws = torch.empty(nbytes, dtype=torch.uint8, device=m.device)

@@ -11,7 +11,7 @@ import typing as T
 
 import torch
 
-from riffusion import _native
+from riffusion import _native, loop_ops
 from riffusion._native import ANY, operand
 
 ACT_NONE, ACT_SILU, ACT_GEGLU, ACT_QUICK_GELU = 0, 1, 2, 3
@@ -101,15 +101,20 @@ def conv2d(
     x: torch.Tensor, w_packed: torch.Tensor, *, x2: T.Optional[torch.Tensor] = None,
     bias: T.Optional[torch.Tensor] = None, bias_per_image: T.Optional[torch.Tensor] = None,
     residual: T.Optional[torch.Tensor] = None, stride: int = 1, act: int = ACT_NONE, pad_far_edge_only: bool = False,
+    wrap_w: bool = False,
 ) -> torch.Tensor:
     """x (and optional x2, concatenated along channels): (B, H, W, C) fp16 NHWC contiguous.
-    w_packed: (Cout, k, k, C1+C2).  Returns (B, Ho, Wo, Cout).  `pad_far_edge_only`: F.pad(x,(0,1,0,1)) + padding=0."""
+    w_packed: (Cout, k, k, C1+C2).  Returns (B, Ho, Wo, Cout).  `pad_far_edge_only`: F.pad(x,(0,1,0,1)) + padding=0.
+    `wrap_w` (3x3, one input): circular padding along W, zeros along H (F.pad(x, (1, 1, 0, 0), mode="circular") +
+    padding=(1, 0)): the convolution reads a bordered copy of x (`loop_ops.pad_wrap_w`) with padding 0."""
     B, H, W, C1 = operand(x, "x", F16, shape=(ANY,) * 4).shape
     dev = x.device
     C2 = 0 if x2 is None else operand(x2, "x2", F16, shape=(B, H, W, ANY), device=dev, layout=None).shape[3]
     Cout, k = operand(w_packed, "w_packed", F16, shape=(ANY, ANY, ANY, C1 + C2), device=dev).shape[:2]
     if w_packed.shape[2] != k:
         raise ValueError(f"w_packed must be (Cout, k, k, C1 + C2), got {tuple(w_packed.shape)}")
+    if wrap_w and (k != 3 or x2 is not None or pad_far_edge_only):
+        raise ValueError("wrap_w takes a 3x3 convolution of one input with symmetric padding")
     pad = 1 if (k == 3 and not pad_far_edge_only) else 0
     extra = 1 if (k == 3 and pad_far_edge_only) else 0
     Ho, Wo = (H + 2 * pad + extra - k) // stride + 1, (W + 2 * pad + extra - k) // stride + 1
@@ -117,6 +122,9 @@ def conv2d(
     d = _native.ConvDesc()
     d.B, d.H, d.W, d.C1, d.C2, d.Cout, d.ksize, d.stride = B, H, W, C1, C2, Cout, k, stride
     d.x1 = x.data_ptr()
+    if wrap_w:
+        xh = loop_ops.pad_wrap_w(x)     # kept alive until the launch is enqueued
+        d.H, d.W, d.x1 = H + 2, W + 2, xh.data_ptr()
     d.x2 = None if x2 is None else x2.contiguous().data_ptr()
     d.w = w_packed.data_ptr()
     d.bias = None if bias is None else operand(bias, "bias", F16, shape=(Cout,), device=dev).data_ptr()
@@ -126,7 +134,7 @@ def conv2d(
         d.bias_per_image_pitch = bias_per_image.stride(0)
     if residual is not None:
         d.residual = operand(residual, "residual", F16, shape=out.shape, device=dev).data_ptr()
-    d.out, d.alpha, d.act, d.pad_mode = out.data_ptr(), 1.0, int(act), int(pad_far_edge_only)
+    d.out, d.alpha, d.act, d.pad_mode = out.data_ptr(), 1.0, int(act), 3 if wrap_w else int(pad_far_edge_only)
     ws = _workspace(_native.lib().rf_conv2d_workspace_bytes(C.byref(d)), d, dev)
     _native.call("rf_conv2d_f16", dev, C.byref(d))
     del ws
@@ -155,9 +163,11 @@ def pack_upsample_weight(w: torch.Tensor) -> torch.Tensor:
     return out.to(torch.float16).contiguous()
 
 
-def conv2d_upsample2x(x: torch.Tensor, w_phases: torch.Tensor, *, bias: T.Optional[torch.Tensor] = None) -> torch.Tensor:
+def conv2d_upsample2x(x: torch.Tensor, w_phases: torch.Tensor, *, bias: T.Optional[torch.Tensor] = None,
+                      wrap_w: bool = False) -> torch.Tensor:
     """conv3x3(pad 1)(nearest_upsample_2x(x)) without materialising the upsampled tensor and with 4/9 of the FLOPs.
-    x: (B, H, W, C) NHWC fp16; w_phases from `pack_upsample_weight`; returns (B, 2H, 2W, Cout)."""
+    x: (B, H, W, C) NHWC fp16; w_phases from `pack_upsample_weight`; returns (B, 2H, 2W, Cout).  `wrap_w`: the 3x3
+    convolution pads circularly along W (the upsampled image wraps where x wraps), reading a bordered copy of x."""
     B, H, W, Cin = operand(x, "x", F16, shape=(ANY,) * 4).shape
     dev = x.device
     Cout = operand(w_phases, "w_phases", F16, shape=(4, ANY, 2, 2, Cin), device=dev).shape[1]
@@ -165,8 +175,11 @@ def conv2d_upsample2x(x: torch.Tensor, w_phases: torch.Tensor, *, bias: T.Option
     d = _native.ConvDesc()
     d.B, d.H, d.W, d.C1, d.C2, d.Cout, d.ksize, d.stride = B, H, W, Cin, 0, Cout, 2, 1
     d.x1, d.x2, d.w = x.data_ptr(), None, w_phases.data_ptr()
+    if wrap_w:
+        xh = loop_ops.pad_wrap_w(x)     # kept alive until the launches are enqueued
+        d.H, d.W, d.x1 = H + 2, W + 2, xh.data_ptr()
     d.bias = None if bias is None else operand(bias, "bias", F16, shape=(Cout,), device=dev).data_ptr()
-    d.out, d.alpha, d.act, d.pad_mode = out.data_ptr(), 1.0, ACT_NONE, 2
+    d.out, d.alpha, d.act, d.pad_mode = out.data_ptr(), 1.0, ACT_NONE, 4 if wrap_w else 2
     _native.call("rf_conv2d_f16", dev, C.byref(d))
     return out
 
@@ -228,8 +241,11 @@ def upsample2x(x: torch.Tensor) -> torch.Tensor:
     return y
 
 
-def conv_in(x_nchw: torch.Tensor, w: torch.Tensor, bias: torch.Tensor) -> torch.Tensor:
-    """(B, Cin<=8, H, W) NCHW fp16 -> (B, H, W, Cout) NHWC; w: torch layout (Cout, Cin, 3, 3) fp16."""
+def conv_in(x_nchw: torch.Tensor, w: torch.Tensor, bias: torch.Tensor, wrap_w: bool = False) -> torch.Tensor:
+    """(B, Cin<=8, H, W) NCHW fp16 -> (B, H, W, Cout) NHWC; w: torch layout (Cout, Cin, 3, 3) fp16.  `wrap_w`: circular
+    padding along W, zeros along H."""
+    if wrap_w:
+        return loop_ops.conv_in_wrap(x_nchw, w, bias)
     B, Cin, H, W = operand(x_nchw, "x", F16, shape=(ANY,) * 4, layout=None).shape
     dev = x_nchw.device
     Cout = operand(w, "w", F16, shape=(ANY, Cin, 3, 3), device=dev).shape[0]
@@ -240,8 +256,11 @@ def conv_in(x_nchw: torch.Tensor, w: torch.Tensor, bias: torch.Tensor) -> torch.
     return y
 
 
-def conv_out(x_nhwc: torch.Tensor, w_packed: torch.Tensor, bias: torch.Tensor) -> torch.Tensor:
-    """(B, H, W, Cin) NHWC -> (B, Cout<=8, H, W) NCHW; w_packed: (Cout, 3, 3, Cin)."""
+def conv_out(x_nhwc: torch.Tensor, w_packed: torch.Tensor, bias: torch.Tensor, wrap_w: bool = False) -> torch.Tensor:
+    """(B, H, W, Cin) NHWC -> (B, Cout<=8, H, W) NCHW; w_packed: (Cout, 3, 3, Cin).  `wrap_w`: circular padding along W,
+    zeros along H."""
+    if wrap_w:
+        return loop_ops.conv_out_wrap(x_nhwc, w_packed, bias)
     B, H, W, Cin = operand(x_nhwc, "x", F16, shape=(ANY,) * 4).shape
     dev = x_nhwc.device
     Cout = operand(w_packed, "w_packed", F16, shape=(ANY, 3, 3, Cin), device=dev).shape[0]

@@ -74,16 +74,17 @@ class UNetB200:
 
     # ------------------------------------------------------------------ building blocks
     def _resnet(self, pfx: str, x: torch.Tensor, st: T.Optional[torch.Tensor], eps: float = 1e-5,
-                skip: T.Optional[torch.Tensor] = None) -> torch.Tensor:
+                skip: T.Optional[torch.Tensor] = None, wrap_w: bool = False) -> torch.Tensor:
         """`skip`: the resnet's input is torch.cat([x, skip], dim=1) (up blocks); the concatenation is never materialised:
-        norm1 reads both tensors in place and the 1x1 shortcut convolution takes them through its two tensor maps."""
+        norm1 reads both tensors in place and the 1x1 shortcut convolution takes them through its two tensor maps.
+        `wrap_w`: the two 3x3 convolutions pad circularly along W."""
         w = self.w
         h = ops.group_norm(x, w[pfx + "norm1.weight"], w[pfx + "norm1.bias"], self.groups, eps, silu=True, x2=skip)
         tproj = None
         if st is not None and pfx in self._temb_slices:
             a, b = self._temb_slices[pfx]
             tproj = self._temb_all[:, a:b]
-        h = ops.conv2d(h, w[pfx + "conv1.weight"], bias=w[pfx + "conv1.bias"], bias_per_image=tproj)
+        h = ops.conv2d(h, w[pfx + "conv1.weight"], bias=w[pfx + "conv1.bias"], bias_per_image=tproj, wrap_w=wrap_w)
         h = ops.group_norm(h, w[pfx + "norm2.weight"], w[pfx + "norm2.bias"], self.groups, eps, silu=True)
         if skip is not None:                        # every concatenating resnet changes the channel count: shortcut exists
             wsc = w[pfx + "conv_shortcut.weight"]
@@ -92,14 +93,15 @@ class UNetB200:
             B, H, W, C = x.shape
             sc = ops.gemm(x.reshape(B * H * W, C), w[pfx + "conv_shortcut.weight"], bias=w[pfx + "conv_shortcut.bias"])
             x = sc.reshape(B, H, W, -1)
-        return ops.conv2d(h, w[pfx + "conv2.weight"], bias=w[pfx + "conv2.bias"], residual=x)
+        return ops.conv2d(h, w[pfx + "conv2.weight"], bias=w[pfx + "conv2.bias"], residual=x, wrap_w=wrap_w)
 
-    def _upsample_conv(self, pfx: str, x: torch.Tensor) -> torch.Tensor:
-        """Upsample2D: F.interpolate(scale_factor=2, mode="nearest") then conv 3x3 pad 1"""
+    def _upsample_conv(self, pfx: str, x: torch.Tensor, wrap_w: bool = False) -> torch.Tensor:
+        """Upsample2D: F.interpolate(scale_factor=2, mode="nearest") then conv 3x3 pad 1 (circular along W with
+        `wrap_w`)"""
         w = self.w
         if self.fused_upsample and x.shape[-1] % 64 == 0:
-            return ops.conv2d_upsample2x(x, w[pfx + "weight.up2x"], bias=w[pfx + "bias"])
-        return ops.conv2d(ops.upsample2x(x), w[pfx + "weight"], bias=w[pfx + "bias"])
+            return ops.conv2d_upsample2x(x, w[pfx + "weight.up2x"], bias=w[pfx + "bias"], wrap_w=wrap_w)
+        return ops.conv2d(ops.upsample2x(x), w[pfx + "weight"], bias=w[pfx + "bias"], wrap_w=wrap_w)
 
     def _attention(self, q: torch.Tensor, k: torch.Tensor, vt: torch.Tensor, nk: int) -> torch.Tensor:
         """q: (B, Nq, C), k: (B, Nk, C), vt: (B, C, pitch>=Nk) (V transposed).  softmax(q k^T / sqrt(d)) v per head,
@@ -174,10 +176,12 @@ class UNetB200:
 
     # ------------------------------------------------------------------ forward
     def forward(self, sample: torch.Tensor, timestep, encoder_hidden_states: torch.Tensor,
-                ctx_cache: T.Optional[dict] = None) -> _Out:
+                ctx_cache: T.Optional[dict] = None, wrap_w: bool = False) -> _Out:
         """sample: (B, 4, H, W) fp16 NCHW; timestep: int / 0-dim / (B,) tensor; encoder_hidden_states: (B, 77, 768).
         `ctx_cache`: a dict that may be reused across calls with the SAME encoder_hidden_states to skip the
-        cross-attention K/V projections (they do not depend on the latents or the timestep)."""
+        cross-attention K/V projections (they do not depend on the latents or the timestep).
+        `wrap_w` (seamless loops): every 3x3 convolution pads circularly along W and with zeros along H, so the output
+        tiles horizontally when the input does.  The 1x1 convolutions, norms and attention do not depend on position."""
         w = self.w
         dev = self.device
         x_in = sample.to(device=dev, dtype=torch.float16)
@@ -193,38 +197,39 @@ class UNetB200:
         st = ops.silu(e2.reshape(B, -1))                       # every resnet applies SiLU to temb first
         self._temb_all = ops.gemm(st, self._temb_w, bias=self._temb_b).reshape(B, -1)
 
-        x = ops.conv_in(x_in, w["conv_in.weight"], w["conv_in.bias"])
+        x = ops.conv_in(x_in, w["conv_in.weight"], w["conv_in.bias"], wrap_w=wrap_w)
         skips = [x]
         n_levels = len(self.c)
         for i in range(n_levels):
             p = f"down_blocks.{i}."
             has_attn = (p + "attentions.0.norm.weight") in w
             for j in range(2):
-                x = self._resnet(f"{p}resnets.{j}.", x, st)
+                x = self._resnet(f"{p}resnets.{j}.", x, st, wrap_w=wrap_w)
                 if has_attn:
                     x = self._transformer(f"{p}attentions.{j}.", x, ctx, ctx_cache)
                 skips.append(x)
             if (p + "downsamplers.0.conv.weight") in w:
-                x = ops.conv2d(x, w[p + "downsamplers.0.conv.weight"], bias=w[p + "downsamplers.0.conv.bias"], stride=2)
+                x = ops.conv2d(x, w[p + "downsamplers.0.conv.weight"], bias=w[p + "downsamplers.0.conv.bias"], stride=2,
+                               wrap_w=wrap_w)
                 skips.append(x)
-        x = self._resnet("mid_block.resnets.0.", x, st)
+        x = self._resnet("mid_block.resnets.0.", x, st, wrap_w=wrap_w)
         x = self._transformer("mid_block.attentions.0.", x, ctx, ctx_cache)
-        x = self._resnet("mid_block.resnets.1.", x, st)
+        x = self._resnet("mid_block.resnets.1.", x, st, wrap_w=wrap_w)
         for i in range(n_levels):
             p = f"up_blocks.{i}."
             has_attn = (p + "attentions.0.norm.weight") in w
             for j in range(3):
-                x = self._resnet(f"{p}resnets.{j}.", x, st, skip=skips.pop())    # torch.cat([x, skip], dim=1) folded in
+                x = self._resnet(f"{p}resnets.{j}.", x, st, skip=skips.pop(), wrap_w=wrap_w)   # torch.cat([x, skip], 1) folded in
                 if has_attn:
                     x = self._transformer(f"{p}attentions.{j}.", x, ctx, ctx_cache)
             if (p + "upsamplers.0.conv.weight") in w:
-                x = self._upsample_conv(p + "upsamplers.0.conv.", x)
+                x = self._upsample_conv(p + "upsamplers.0.conv.", x, wrap_w=wrap_w)
         x = ops.group_norm(x, w["conv_norm_out.weight"], w["conv_norm_out.bias"], self.groups, 1e-5, silu=True)
-        out = ops.conv_out(x, w["conv_out.weight"], w["conv_out.bias"])
+        out = ops.conv_out(x, w["conv_out.weight"], w["conv_out.bias"], wrap_w=wrap_w)
         return _Out(sample=out)
 
     def __call__(self, latent_model_input, t, encoder_hidden_states=None, **kw):
-        return self.forward(latent_model_input, t, encoder_hidden_states, kw.get("ctx_cache"))
+        return self.forward(latent_model_input, t, encoder_hidden_states, kw.get("ctx_cache"), kw.get("wrap_w", False))
 
     # diffusers-like conveniences used by pipeline code
     def to(self, *a, **k):

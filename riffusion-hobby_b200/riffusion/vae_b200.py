@@ -54,29 +54,31 @@ class VaeB200(UNetB200):
                        residual=x.reshape(rows, C))
         return out.reshape(B, H, W, C)
 
-    def _mid(self, pfx: str, x: torch.Tensor) -> torch.Tensor:
-        x = self._resnet(pfx + "resnets.0.", x, None, eps=1e-6)
+    def _mid(self, pfx: str, x: torch.Tensor, wrap_w: bool = False) -> torch.Tensor:
+        x = self._resnet(pfx + "resnets.0.", x, None, eps=1e-6, wrap_w=wrap_w)
         x = self._attn_block(pfx + "attentions.0.", x)
-        return self._resnet(pfx + "resnets.1.", x, None, eps=1e-6)
+        return self._resnet(pfx + "resnets.1.", x, None, eps=1e-6, wrap_w=wrap_w)
 
     # -- decode ------------------------------------------------------------------------------------------
-    def decode(self, z: torch.Tensor, scale: float = 1.0):
+    def decode(self, z: torch.Tensor, scale: float = 1.0, wrap_w: bool = False):
         """z: (B, 4, h, w) fp16 NCHW latents (already divided by 0.18215 unless `scale` folds it in).
-        Returns an object with `.sample`: (B, 3, 8h, 8w) fp16 NCHW in [-1, 1]."""
+        Returns an object with `.sample`: (B, 3, 8h, 8w) fp16 NCHW in [-1, 1].  `wrap_w` (seamless loops): every 3x3
+        convolution pads circularly along W, so the image tiles horizontally when the latents do."""
         w = self.w
         z = z.to(device=self.device, dtype=torch.float16)
         z = ops.conv1x1_small(z, w["post_quant_conv.weight"], w["post_quant_conv.bias"], in_scale=scale)
-        x = ops.conv_in(z, w["decoder.conv_in.weight"], w["decoder.conv_in.bias"])
-        x = self._mid("decoder.mid_block.", x)
+        x = ops.conv_in(z, w["decoder.conv_in.weight"], w["decoder.conv_in.bias"], wrap_w=wrap_w)
+        x = self._mid("decoder.mid_block.", x, wrap_w=wrap_w)
         n = len(self.c)
         for i in range(n):
             p = f"decoder.up_blocks.{i}."
             for j in range(3):
-                x = self._resnet(f"{p}resnets.{j}.", x, None, eps=1e-6)
+                x = self._resnet(f"{p}resnets.{j}.", x, None, eps=1e-6, wrap_w=wrap_w)
             if (p + "upsamplers.0.conv.weight") in w:
-                x = self._upsample_conv(p + "upsamplers.0.conv.", x)
+                x = self._upsample_conv(p + "upsamplers.0.conv.", x, wrap_w=wrap_w)
         x = ops.group_norm(x, w["decoder.conv_norm_out.weight"], w["decoder.conv_norm_out.bias"], self.groups, 1e-6, silu=True)
-        return types.SimpleNamespace(sample=ops.conv_out(x, w["decoder.conv_out.weight"], w["decoder.conv_out.bias"]))
+        return types.SimpleNamespace(sample=ops.conv_out(x, w["decoder.conv_out.weight"], w["decoder.conv_out.bias"],
+                                                         wrap_w=wrap_w))
 
     # -- encode ------------------------------------------------------------------------------------------
     def encode_moments(self, image: torch.Tensor) -> T.Tuple[torch.Tensor, torch.Tensor]:
