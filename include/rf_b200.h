@@ -376,6 +376,17 @@ int rf_axpby_f16(const void* x, const void* noise, float a, float b, const void*
  *   rounding of u; mix = 1 returns x bit for bit, mix = 0 is the plain noising of enc. */
 int rf_magic_mix_f16(const void* x, const void* enc, const float* noise, float a, float b, float mix, long n, void* u,
                      void* stream);
+/* Long tracks (MultiDiffusion): n windows of Ww columns at stride s over a canvas of Wc = Ww + (n - 1) s columns.  Rows
+ * are NCHW fp16; G groups of rows (the [uncond | text] halves of the tracks, track-major, or the tracks without CFG).
+ * Ww, s and Wc are multiples of 8 with 0 < s <= Ww; pointers 16-byte aligned.
+ *   gather: canvas [G][C][H][Wc] -> windows [G*n][C][H][Ww], windows[g*n + k][c][y][x] = canvas[g][c][y][k*s + x], a copy.
+ *   merge:  windows [G*n][C][H][Ww] + d_weights fp32 DEVICE [n][Ww] -> canvas [G][C][H][Wc],
+ *           canvas[g][c][y][X] = fp16(sum over the windows k that cover X, in increasing k, of
+ *           d_weights[k][X - k*s] * windows[g*n + k][c][y][X - k*s]), fp32 accumulation, one rounding, no atomics. */
+int rf_window_gather_f16(const void* canvas, int G, int C, int H, int Wc, int Ww, int s, int n, void* windows,
+                         void* stream);
+int rf_window_merge_f16(const void* windows, const float* d_weights, int G, int C, int H, int Wc, int Ww, int s, int n,
+                        void* canvas, void* stream);
 
 #ifdef __cplusplus
 }

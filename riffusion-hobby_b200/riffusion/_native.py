@@ -144,6 +144,10 @@ SIGNATURES = {
                                C.c_void_p, C.c_void_p]),
     "rf_magic_mix_f16": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_float, C.c_float, C.c_float, C.c_long,
                                    C.c_void_p, C.c_void_p]),
+    "rf_window_gather_f16": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
+                                       C.c_void_p, C.c_void_p]),
+    "rf_window_merge_f16": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
+                                      C.c_int, C.c_void_p, C.c_void_p]),
     "rf_attention_masked_f16": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int,
                                    C.c_int, C.c_int, C.c_float, C.c_int, C.c_void_p]),
     "rf_tc_profile_begin": (C.c_int, []),

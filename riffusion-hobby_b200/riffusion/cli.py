@@ -21,6 +21,10 @@ the same names, flags and defaults (`COMMANDS`, what `build_parser()` builds by 
         [--image-dir steps] [--seed-a 42] [--seed-b 42] [--denoising-a 0.75] [--denoising-b 0.75] [--guidance 7.0]
         [--num-interpolation-steps 12] [--num-inference-steps 50] [--alpha-power 1.0] [--max-batch 32]
         [--checkpoint DIR] [--device cuda]
+    python -m riffusion.cli text-to-track --prompt "lo-fi piano" --audio out.wav [--image out.png]
+        [--prompt-changes "20:jazz with drums;40:hard rock"] [--negative-prompt ...] [--duration-s 30] [--seed 42]
+        [--num-tracks 1] [--num-inference-steps 30] [--guidance 7.0] [--scheduler DPMSolverMultistepScheduler]
+        [--window-width 512] [--stride 256] [--max-batch 32] [--use-20k] [--checkpoint DIR] [--device cuda]
     python -m riffusion.cli text-to-audio-batch --json inputs.json --output-dir out [--num-seeds 1] [--max-batch 32]
         [--audio-extension wav] [--checkpoint DIR] [--device cuda]
 
@@ -240,6 +244,62 @@ def text_to_audio(*, prompt: str, audio: str, image: str = "", negative_prompt: 
             print(f"Wrote {img_path}")
 
 
+def parse_prompt_changes(prompt: str, changes: str) -> T.Union[str, T.List[T.Tuple[float, str]]]:
+    """--prompt and --prompt-changes "20:jazz with drums;40:hard rock" -> [(0, prompt), (20, ...), (40, ...)], or the
+    prompt alone without changes.  ValueError for an entry that is not <seconds>:<prompt>."""
+    if not changes.strip():
+        return prompt
+    spans: T.List[T.Tuple[float, str]] = [(0.0, prompt)]
+    for entry in changes.split(";"):
+        start, sep, text = entry.partition(":")
+        try:
+            at = float(start) if sep else float("nan")
+        except ValueError:
+            at = float("nan")
+        if not sep or at != at or not text.strip():
+            raise ValueError(f"--prompt-changes entry {entry!r} is not <seconds>:<prompt>")
+        spans.append((at, text.strip()))
+    return spans
+
+
+def text_to_track(*, prompt: str, audio: str, image: str = "", prompt_changes: str = "", negative_prompt: str = "",
+                  duration_s: float = 30.0, seed: int = 42, num_tracks: int = 1, num_inference_steps: int = 30,
+                  guidance: float = 7.0, scheduler: str = "DPMSolverMultistepScheduler", window_width: int = 512,
+                  stride: int = 256, max_batch: int = 32, use_20k: bool = False,
+                  checkpoint: str = "riffusion/riffusion-model-v1", device: str = "cuda"):
+    """Generate a long track from text: overlapping clip windows denoised as one canvas (--window-width, --stride);
+    --prompt-changes "20:jazz with drums;40:hard rock" switches the prompt at those times (seconds)."""
+    from riffusion.riffusion_pipeline import RiffusionPipeline
+    from riffusion.util import audio_util
+
+    params = _app_params(use_20k)
+    spans = parse_prompt_changes(prompt, prompt_changes)
+    RiffusionPipeline.track_geometry(duration_s, window_width, stride, params.hop_length, params.sample_rate)
+    RiffusionPipeline.track_prompts(spans, 1, window_width, stride, params.hop_length, params.sample_rate)
+    pipe = RiffusionPipeline.load_checkpoint(checkpoint=checkpoint, device=device)
+    out = pipe.text_to_track(spans, duration_s=duration_s, params=params, window_width=window_width, stride=stride,
+                             negative_prompt=negative_prompt or None, seed=seed, num_tracks=num_tracks,
+                             num_inference_steps=num_inference_steps, guidance_scale=guidance, scheduler=scheduler,
+                             max_batch=max_batch)
+    images, waves = out["images"].cpu().numpy(), out["waveform"].cpu().numpy()
+
+    def target(path: str, i: int) -> Path:
+        p = Path(path)
+        return p if num_tracks == 1 else p.with_name(f"{p.stem}_{seed + i}{p.suffix}")
+
+    for i in range(num_tracks):
+        segment = audio_util.apply_filters(
+            audio_util.audio_from_waveform(samples=waves[i], sample_rate=params.sample_rate, normalize=True),
+            compression=False)
+        wav_path = target(audio, i)
+        segment.export(str(wav_path), format=wav_path.suffix[1:])
+        print(f"Wrote {wav_path} ({segment.duration_seconds:.2f} seconds, {len(out['windows'])} windows)")
+        if image:
+            img_path = target(image, i)
+            _store_spectrogram(images[i], params, img_path, _PIL_FORMAT.get(img_path.suffix[1:].lower(), "PNG"))
+            print(f"Wrote {img_path}")
+
+
 def audio_to_audio(*, audio: str, output: str, prompt: str, image_dir: str = "", negative_prompt: str = "",
                    seed: int = 42, denoising: float = 0.55, num_inference_steps: int = 25, guidance: float = 7.0,
                    scheduler: str = "DPMSolverMultistepScheduler", start_time_s: float = 0.0, duration_s: float = 20.0,
@@ -335,7 +395,7 @@ COMMANDS = [audio_to_image, image_to_audio, sample_clips, print_exif, audio_to_i
 # commands of this package that the reference's CLI does not have; `main` offers them next to COMMANDS
 EXTRA_COMMANDS = [text_to_audio]
 # the track-level commands, offered by `main` after EXTRA_COMMANDS
-TRACK_COMMANDS = [audio_to_audio, interpolation]
+TRACK_COMMANDS = [audio_to_audio, interpolation, text_to_track]
 # the file-driven batch commands, offered by `main` after TRACK_COMMANDS
 BATCH_COMMANDS = [text_to_audio_batch]
 

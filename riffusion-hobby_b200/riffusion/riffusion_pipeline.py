@@ -15,6 +15,7 @@ encoder is supplied, otherwise callers pass text embeddings directly.
 from __future__ import annotations
 
 import functools
+import math
 import typing as T
 from pathlib import Path
 
@@ -23,6 +24,7 @@ import torch
 from PIL import Image
 
 from riffusion import tc_ops as ops
+from riffusion import window_ops
 from riffusion.datatypes import InferenceInput
 from riffusion.scheduler_b200 import (DDIMSchedulerB200, EulerAncestralSchedulerB200, PNDMSchedulerB200,
                                       make_scheduler)
@@ -636,7 +638,7 @@ class RiffusionPipeline:
                  mask: T.Optional[torch.Tensor] = None, init: T.Optional[torch.Tensor] = None,
                  noise: T.Optional[torch.Tensor] = None,
                  layout: T.Optional[T.Tuple[float, torch.Tensor, torch.Tensor, int]] = None,
-                 wrap_w: bool = False) -> T.Tuple[torch.Tensor, int]:
+                 wrap_w: bool = False, windows: T.Optional[window_ops.Windows] = None) -> T.Tuple[torch.Tensor, int]:
         """The CFG loop over `timesteps`: one UNet evaluation of [latents | latents] (a captured CUDA graph when enabled)
         and one fused guidance + scheduler step each.  With a `mask`, every step is followed by the inpainting blend of
         interpolate_img2img (:420-425): `init` noised with `noise` at that step's timestep where the mask is 1, the
@@ -645,12 +647,18 @@ class RiffusionPipeline:
         noise32, t) (`tc_ops.magic_mix`) and the scheduler still steps the latents.  The UNet input passes through
         `sched.scale_model_input` (the identity, without a launch, for every scheduler but Euler ancestral).  The UNet,
         the graph and the scheduler receive the scheduler's own timestep values: ints, or floats for Euler ancestral.
-        `wrap_w`: the UNet pads circularly along W (seamless loops).  Returns (latents, evaluations)."""
+        `wrap_w`: the UNet pads circularly along W (seamless loops).  `windows` (long tracks): `latents` is a canvas of
+        `windows.canvas` columns; each step gathers its windows (`window_ops.window_gather`), evaluates the UNet on them
+        (context: one row per window, track-major) and merges both halves of the eps pair back onto the canvas
+        (`window_ops.window_merge`) before the scheduler steps the canvas.  Returns (latents, evaluations)."""
         do_cfg = guidance_scale > 1.0
         ctx_cache: T.Dict[str, T.Any] = {}
         graphed = None
+        unet_shape = latents.shape
+        if windows is not None:
+            unet_shape = (latents.shape[0] * windows.n,) + tuple(latents.shape[1:3]) + (windows.width,)
         if do_cfg:
-            graphed = self._graphed_unet(latents.shape, context, True) if wrap_w else self._graphed_unet(latents.shape, context)
+            graphed = self._graphed_unet(unet_shape, context, True) if wrap_w else self._graphed_unet(unet_shape, context)
         loop_kw = dict(wrap_w=True) if wrap_w else {}
         if mask is not None:
             mask = mask.to(device=latents.device, dtype=latents.dtype).expand_as(latents).contiguous()
@@ -662,11 +670,15 @@ class RiffusionPipeline:
                 a = float(sched.alphas_cumprod[t_val])
                 unet_in = ops.magic_mix(latents, layout[1], layout[2], a ** 0.5, (1.0 - a) ** 0.5, layout[0])
             unet_in = sched.scale_model_input(unet_in, t_val)
+            if windows is not None:
+                unet_in = window_ops.window_gather(unet_in, windows)
             if graphed is not None:
                 eps_pair = graphed(unet_in, t_val)
             else:
                 model_in = torch.cat([unet_in] * 2) if do_cfg else unet_in
                 eps_pair = self.unet(model_in, t_val, encoder_hidden_states=context, ctx_cache=ctx_cache, **loop_kw).sample
+            if windows is not None:
+                eps_pair = window_ops.window_merge(eps_pair, windows)
             n_evals += 1
             if not do_cfg:
                 eps_pair = torch.cat([eps_pair, eps_pair])
@@ -868,6 +880,168 @@ class RiffusionPipeline:
             wave = self._u8_to_waveform(u8, converter, params.stereo, init_angles)
         return dict(images=u8, waveform=wave, latents=out["latents"], latents_unscaled=out["latents_unscaled"],
                     n_unet_evals=out["n_unet_evals"])
+
+    # ------------------------------------------------------------------------------ long tracks
+    @staticmethod
+    def track_loops(num_tracks: int, n_windows: int, max_batch: int) -> T.List[T.List[int]]:
+        """The tracks of each CFG loop of `txt2img_track`, in order: as many whole tracks as fit in `max_batch` windows,
+        at least one per loop (a track is never split)."""
+        if num_tracks < 1:
+            raise ValueError("num_tracks must be at least 1")
+        if max_batch < 1:
+            raise ValueError("max_batch must be at least 1")
+        per = max(1, max_batch // n_windows)
+        return [list(range(lo, min(num_tracks, lo + per))) for lo in range(0, num_tracks, per)]
+
+    @torch.no_grad()
+    def txt2img_track(self, prompt: T.Union[str, T.Sequence[str]], *, width: int, height: int = 512,
+                      window_width: int = 512, stride: int = 256, negative_prompt: T.Optional[str] = None, seed: int = 42,
+                      num_tracks: int = 1, num_inference_steps: int = 30, guidance_scale: float = 7.0,
+                      scheduler: str = "DPMSolverMultistepScheduler", max_batch: int = 32,
+                      output_type: T.Optional[str] = "pil", text_embeddings: T.Optional[torch.Tensor] = None,
+                      uncond_embeddings: T.Optional[torch.Tensor] = None, latents: T.Optional[torch.Tensor] = None,
+                      step_noise: T.Optional[torch.Tensor] = None) -> T.Dict[str, T.Any]:
+        """`txt2img` of a canvas wider than the model, MultiDiffusion style (Bar-Tal et al. 2023): the canvas of `width`
+        pixels is denoised as n = (width - window_width) / stride + 1 overlapping windows of `window_width` pixels.  Every
+        step gathers the windows, runs the UNet on them at its trained size, merges the [uncond | text] eps of the
+        windows onto the canvas with the crossfade weights of `window_ops.merge_weights`, and steps the canvas with the
+        scheduler's own fused guidance + update (`_denoise` with `windows`).
+
+        `prompt` is one string, or one per window (window k's text context); the prompts and the negative prompt
+        (default "") are embedded without weighting.  Track i starts from txt2img's draw at `width` for seed + i, and
+        Euler ancestral draws txt2img's per-step noise.  Tracks share loops in order (`track_loops`), so the UNet batch
+        is twice the windows of a loop.  `text_embeddings` (1 or n rows) / `uncond_embeddings` / `latents` (num_tracks,
+        4, height/8, width/8) / `step_noise` (steps, num_tracks, 4, height/8, width/8) replace the text encoder and the
+        generator draws.  With one window the call is `txt2img` at that width.
+
+        Raises ValueError before any device work unless width, window_width, stride and height are positive multiples
+        of 64 with 0 < stride <= window_width and width = window_width + (n - 1) stride, for a prompt list that is not one
+        per window, num_tracks or max_batch below 1, or an unknown scheduler.  Returns txt2img's dict (n_unet_evals:
+        the UNet evaluations of all loops) plus windows (the window offsets in pixels) and loops (the tracks of each
+        loop)."""
+        n = window_ops.window_count(width, window_width, stride)
+        if height <= 0 or height % 64:
+            raise ValueError(f"height must be a positive multiple of 64, got {height}")
+        prompts = [prompt] * n if isinstance(prompt, str) else list(prompt)
+        if len(prompts) != n:
+            raise ValueError(f"{len(prompts)} prompts for {n} windows: give one prompt, or one per window")
+        loops = self.track_loops(num_tracks, n, max_batch)
+        make_scheduler(scheduler)
+        dev = self._device
+        win = window_ops.Windows.make(window_width // 8, stride // 8, n, dev)
+        if text_embeddings is None:
+            embedded = {p: self.embed_text(p) for p in dict.fromkeys(prompts)}
+            text_embeddings = torch.cat([embedded[p] for p in prompts])
+        texts = text_embeddings.to(device=dev, dtype=torch.float16)
+        texts = texts.expand(n, -1, -1) if texts.shape[0] == 1 else texts
+        if texts.shape[0] != n:
+            raise ValueError(f"text_embeddings hold {texts.shape[0]} rows for {n} windows")
+        shape = (1, 4, height // 8, width // 8)
+        gens = [torch.Generator(device=self.device).manual_seed(seed + i) for i in range(num_tracks)]
+        if latents is None:
+            latents = torch.cat([torch.randn(shape, generator=g, device=self.device, dtype=torch.float16) for g in gens])
+        latents = latents.to(device=dev, dtype=torch.float16).contiguous()
+        if tuple(latents.shape) != (num_tracks,) + shape[1:]:
+            raise ValueError(f"latents must be {(num_tracks,) + shape[1:]}, got {tuple(latents.shape)}")
+        outs, n_evals = [], 0
+        for idx in loops:
+            sched = make_scheduler(scheduler)
+            sched.set_timesteps(num_inference_steps)
+            lat = latents[idx[0]:idx[-1] + 1]
+            noise = None if step_noise is None else step_noise[:, idx[0]:idx[-1] + 1]
+            self._step_noise(sched, len(sched.timesteps), lat, noise, [gens[i] for i in idx])
+            if sched.init_noise_sigma != 1.0:
+                lat = (lat * sched.init_noise_sigma).contiguous()
+            context = self._context(None, negative_prompt, len(idx) * n, guidance_scale > 1.0, texts.repeat(len(idx), 1, 1),
+                                    uncond_embeddings)
+            lat, evals = self._denoise(sched, sched.timesteps, lat, context, guidance_scale, windows=win)
+            outs.append(lat)
+            n_evals += evals
+        out = self._finish(torch.cat(outs), n_evals, output_type)
+        out["windows"] = window_ops.window_offsets(n, stride)
+        out["loops"] = loops
+        return out
+
+    @staticmethod
+    def track_geometry(duration_s: float, window_width: int, stride: int, hop_length: int,
+                       sample_rate: int) -> T.Tuple[int, int, int]:
+        """(frames, canvas width, windows) of a `duration_s` track: F = ceil(duration_s sr / hop) + 1 frames on the
+        narrowest canvas of whole strides that holds them (`window_ops.canvas_width`).  ValueError unless 0 < duration_s
+        <= 120 and window_width, stride are positive multiples of 64 with stride <= window_width."""
+        if not 0 < duration_s <= 120:
+            raise ValueError(f"duration_s must be in (0, 120] seconds, got {duration_s}")
+        window_ops.window_count(window_width, window_width, stride)
+        frames = math.ceil(duration_s * sample_rate / hop_length) + 1
+        width = window_ops.canvas_width(frames, window_width, stride)
+        return frames, width, window_ops.window_count(width, window_width, stride)
+
+    @staticmethod
+    def track_prompts(prompt: T.Union[str, T.Sequence[T.Tuple[float, str]]], n_windows: int, window_width: int,
+                      stride: int, hop_length: int, sample_rate: int) -> T.List[str]:
+        """The prompt of each window: `prompt` itself, or from a list of (start_s, prompt) spans, the span in force at
+        the window's centre time (k stride + window_width / 2 frames).  ValueError for an empty list or spans whose first
+        start is not 0 or whose starts do not strictly increase."""
+        if isinstance(prompt, str):
+            return [prompt] * n_windows
+        spans = [(float(s), p) for s, p in prompt]
+        if not spans:
+            raise ValueError("no prompt spans: give a prompt or a list of (start_s, prompt)")
+        if spans[0][0] != 0.0:
+            raise ValueError(f"the first prompt span must start at 0 s, got {spans[0][0]}")
+        for (a, _), (b, _) in zip(spans, spans[1:]):
+            if not b > a:
+                raise ValueError(f"prompt span starts must strictly increase, got {a} then {b}")
+        out = []
+        for k in range(n_windows):
+            centre = (k * stride + window_width / 2) * hop_length / sample_rate
+            out.append([p for s, p in spans if s <= centre][-1])
+        return out
+
+    @torch.no_grad()
+    def text_to_track(self, prompt: T.Union[str, T.Sequence[T.Tuple[float, str]]], *, duration_s: float = 30.0,
+                      params=None, window_width: int = 512, stride: int = 256, negative_prompt: T.Optional[str] = None,
+                      seed: int = 42, num_tracks: int = 1, num_inference_steps: int = 30, guidance_scale: float = 7.0,
+                      scheduler: str = "DPMSolverMultistepScheduler", max_batch: int = 32,
+                      text_embeddings: T.Optional[torch.Tensor] = None, uncond_embeddings: T.Optional[torch.Tensor] = None,
+                      latents: T.Optional[torch.Tensor] = None, step_noise: T.Optional[torch.Tensor] = None,
+                      converter=None, init_angles: T.Optional[torch.Tensor] = None) -> T.Dict[str, T.Any]:
+        """A track of `duration_s` seconds from text: `txt2img_track` at height params.num_frequencies on the canvas of
+        `track_geometry`, then per track on the device: VAE decode -> uint8 image -> mel (`rf_image_to_mel`) -> inverse
+        mel + Griffin-Lim, trimmed to round(duration_s sr) samples.  `params` defaults to mono 0-10 kHz.
+
+        `prompt` is a string or a list of (start_s, prompt) spans (`track_prompts`): each window takes the prompt in force
+        at its centre, so the overlaps crossfade from one prompt to the next.  `init_angles` (num_tracks, channels,
+        n_fft/2 + 1, canvas width) fixes Griffin-Lim's initial phases; the other options are `txt2img_track`'s.
+
+        Raises ValueError before any device work for a duration outside (0, 120] s, bad window geometry, malformed
+        prompt spans, an unknown scheduler, num_tracks or max_batch below 1.  Returns device tensors images
+        (num_tracks, H, canvas width, 3) uint8, waveform (num_tracks, channels, round(duration_s sr)) fp32 before peak
+        normalisation, latents, latents_unscaled, and windows (per window: offset in pixels and prompt), n_unet_evals,
+        loops."""
+        params = DEFAULT_PARAMS if params is None else params
+        hop, sr = params.hop_length, params.sample_rate
+        _, width, n = self.track_geometry(duration_s, window_width, stride, hop, sr)
+        prompts = self.track_prompts(prompt, n, window_width, stride, hop, sr)
+        self.track_loops(num_tracks, n, max_batch)
+        make_scheduler(scheduler)
+        converter = self._converter(params, converter)
+        out = self.txt2img_track(prompts, width=width, height=params.num_frequencies, window_width=window_width,
+                                 stride=stride, negative_prompt=negative_prompt, seed=seed, num_tracks=num_tracks,
+                                 num_inference_steps=num_inference_steps, guidance_scale=guidance_scale,
+                                 scheduler=scheduler, max_batch=max_batch, output_type="latent",
+                                 text_embeddings=text_embeddings, uncond_embeddings=uncond_embeddings, latents=latents,
+                                 step_noise=step_noise)
+        samples = round(duration_s * sr)
+        u8s, waves = [], []
+        for i in range(num_tracks):
+            u8 = self._decode_u8(out["latents"][i:i + 1])
+            angles = None if init_angles is None else init_angles[i:i + 1]
+            waves.append(self._u8_to_waveform(u8, converter, params.stereo, angles)[..., :samples])
+            u8s.append(u8)
+        return dict(images=torch.cat(u8s), waveform=torch.cat(waves), latents=out["latents"],
+                    latents_unscaled=out["latents_unscaled"],
+                    windows=[dict(offset=o, prompt=p) for o, p in zip(out["windows"], prompts)],
+                    n_unet_evals=out["n_unet_evals"], loops=out["loops"])
 
     @torch.no_grad()
     def text_to_audio_batch(self, batch: dict, *, num_seeds: int = 1, max_batch: int = 32, converter=None,

@@ -105,7 +105,9 @@ class UNetB200:
 
     def _attention(self, q: torch.Tensor, k: torch.Tensor, vt: torch.Tensor, nk: int) -> torch.Tensor:
         """q: (B, Nq, C), k: (B, Nk, C), vt: (B, C, pitch>=Nk) (V transposed).  softmax(q k^T / sqrt(d)) v per head,
-        scores materialised in fp16 like the reference's baddbmm/softmax/bmm (diffusers attention)."""
+        scores materialised in fp16 like the reference's baddbmm/softmax/bmm (diffusers attention).  The score buffer of
+        one launch stays within `max_score_bytes`: whole images per launch while one image's scores fit, else one image
+        at a time in chunks of queries (a wide VAE decode)."""
         B, Nq, C = q.shape
         h = self.heads
         d = C // h
@@ -114,6 +116,9 @@ class UNetB200:
         pitch = (nk + 7) // 8 * 8
         out = torch.empty((B, Nq, C), dtype=torch.float16, device=q.device)
         per_b = h * Nq * pitch * 2
+        if per_b > self.max_score_bytes:
+            self._attention_query_chunks(q, k, vt, nk, out)
+            return out
         chunk = max(1, min(B, self.max_score_bytes // max(per_b, 1)))
         for b0 in range(0, B, chunk):
             b1 = min(B, b0 + chunk)
@@ -126,6 +131,27 @@ class UNetB200:
             ov = out[b0:b1].view(b1 - b0, Nq, h, d).permute(0, 2, 1, 3)
             ops.gemm(s[..., :nk], vv, out=ov)
         return out
+
+    def _attention_query_chunks(self, q: torch.Tensor, k: torch.Tensor, vt: torch.Tensor, nk: int,
+                                out: torch.Tensor) -> None:
+        """`_attention`'s materialised path for images whose (heads, Nq, pitch) score block exceeds `max_score_bytes`:
+        per image, queries in chunks of a multiple of 64 rows whose scores fit.  A query row's scores, softmax and output
+        do not depend on the other rows, so only the launch shapes change."""
+        B, Nq, C = q.shape
+        h = self.heads
+        d = C // h
+        pitch = (nk + 7) // 8 * 8
+        rows = max(64, self.max_score_bytes // (h * pitch * 2) // 64 * 64)
+        for b in range(B):
+            kv = k[b:b + 1].view(1, nk, h, d).permute(0, 2, 1, 3)
+            vv = vt[b:b + 1].view(1, h, d, vt.shape[-1])[..., :nk]
+            for q0 in range(0, Nq, rows):
+                q1 = min(Nq, q0 + rows)
+                sc = torch.empty((1, h, q1 - q0, pitch), dtype=torch.float16, device=q.device)
+                qv = q[b:b + 1, q0:q1].view(1, q1 - q0, h, d).permute(0, 2, 1, 3)
+                ops.gemm(qv, kv, alpha=d ** -0.5, out=sc[..., :nk])
+                ops.softmax_rows_(sc, nk)
+                ops.gemm(sc[..., :nk], vv, out=out[b:b + 1, q0:q1].view(1, q1 - q0, h, d).permute(0, 2, 1, 3))
 
     def _kv(self, pfx: str, ctx: torch.Tensor) -> T.Tuple[torch.Tensor, torch.Tensor]:
         """K = ctx Wk^T (B, Nk, C) and V^T = Wv ctx^T (B, C, pitch) — V is produced already transposed by
